@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the Vitron multimodal forward path on B200.
+"""bench.py — headline benchmark of the Vitron multimodal forward path on an H100 (sm_90a).
 
 Workload (BASELINE.json configs[1]): batch-8 images -> LanguageBind ViT-L/14 encode + mlp2x_gelu
 projector + splice -> Vicuna-7B prefill over 256 vision + 512 text tokens -> 128 greedy decode
@@ -9,7 +9,11 @@ batch. `value` = generated tokens / s of the whole job (all ranks) with inputs r
 back. N > 1: one process per GPU (torchrun), independent request batches (weak scaling), one NCCL
 all_gather of the generated ids at the end of every step.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
+
+--steps K sets the timed steps of every leg (tokens/s, e2e, video, UNet). --dump-outputs DIR writes what the timed path
+returned in its last step as DIR/<name>.npy (token ids as float64, latents as float32): the inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -36,8 +40,8 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet (dense bf16, 700 W)"
 
 
 class ClockSampler(threading.Thread):
@@ -249,6 +253,16 @@ def build_model(device):
     return model
 
 
+def dump_outputs(directory, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array; integer results (token ids) as float64, which holds them exactly."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        a = t.float().numpy() if t.is_floating_point() else t.double().numpy()
+        np.save(os.path.join(directory, name + ".npy"), a)
+
+
 def timed(fn, iters):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
@@ -338,7 +352,7 @@ def _unet_inputs(device, seed=4):
 
 
 def unet_gemm_roofline(unet, noise, cond, tf_peak, peak_kind, t_steps=None):
-    """Dominant kernel family of a UNet forward = the tcgen05 GEMM / implicit-GEMM conv kernel (gemm_v2_kernel<BN,...>,
+    """Dominant kernel family of a UNet forward = the wgmma GEMM / implicit-GEMM conv kernel (gemm_v2_kernel<BN,...>,
     ~70 % of the forward). Every ops.gemm / ops.conv_nhwc call of ONE forward is recorded with its live operands, then
     exactly those calls are replayed back to back from a CUDA graph and timed with CUDA events: achieved = their
     algorithmic FLOPs (2*M*N*K, conv 2*pixels*cout*cin*taps) / that time. `noise` / `cond` are what the timed step feeds the
@@ -393,7 +407,7 @@ def unet_gemm_roofline(unet, noise, cond, tf_peak, peak_kind, t_steps=None):
         with open(pj) as fh:
             traffic = json.load(fh).get("traffic_bytes_per_launch")
     ach = flops / (ms * 1e-3) / 1e12
-    return {"bound": "tensor", "kernel": "gemm_v2_kernel<BN,STAGES,EPI> (tcgen05 GEMM + implicit-GEMM conv: every Linear / Conv2d / Conv3d of the forward)",
+    return {"bound": "tensor", "kernel": "gemm_v2_kernel<BN,STAGES,EPI> (wgmma GEMM + implicit-GEMM conv: every Linear / Conv2d / Conv3d of the forward)",
             "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s", "frac": ach / tf_peak,
             "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({peak_kind}, burst)", "traffic": traffic,
             "launches": len(calls), "algorithmic_tflop": flops / 1e12, "avg_launch_us": ms * 1e3 / len(calls), "replay_ms": ms}
@@ -424,7 +438,7 @@ def unet_cpu_baseline():
                       "(frames x pixels) to the [1,4,16,40,64] latent, 2 forwards per step"}
 
 
-def bench_unet(device, tf_peak, peak_kind, steps=10, rank=0, world=1, with_cpu=True):
+def bench_unet(device, tf_peak, peak_kind, steps=10, rank=0, world=1, with_cpu=True, outputs=None):
     """Second half of BASELINE.json's metric: i2vgen-xl UNet3D denoise steps/s (configs[4] at the primary latent reading
     16 x (40x64) = 320x512 px; DDIM step = the conditional and the unconditional UNet evaluation of classifier-free guidance 9.0
     — run as ONE batch-2 forward [cond | uncond], GraphedCFGDenoiser — + the v-prediction update),
@@ -460,7 +474,7 @@ def bench_unet(device, tf_peak, peak_kind, steps=10, rank=0, world=1, with_cpu=T
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.synchronize()
         e0.record()
-        xt = run_steps(model, xt, ts[3:3 + n])
+        xt = run_steps(model, xt, [ts[3 + i % (len(ts) - 3)] for i in range(n)])   # --steps beyond the schedule wrap around
         e1.record()
         torch.cuda.synchronize()
         if world > 1:
@@ -473,6 +487,8 @@ def bench_unet(device, tf_peak, peak_kind, steps=10, rank=0, world=1, with_cpu=T
     l0 = ops.launch_count()
     ms, xt = time_steps(den, noise, steps)
     launches = (ops.launch_count() - l0) // (steps + 3)
+    if outputs is not None:
+        outputs["unet_latent"] = xt
     finite = bool(torch.isfinite(xt).all())
     tfs = 2 * UNET_TFLOP_PER_FORWARD / (ms * 1e-3)
     out = {"metric": UNET_METRIC, "value": world * 1000.0 / ms, "unit": "steps/s", "n_gpus": world, "steps": steps, "warmup": 3,
@@ -480,7 +496,7 @@ def bench_unet(device, tf_peak, peak_kind, steps=10, rank=0, world=1, with_cpu=T
            "config": {"workload": "BASELINE.json configs[4], primary latent reading [1,4,16,40,64]; DDIM-50 schedule, guide 9.0",
                       "parallelism": f"{world} request replica(s)", "requests_in_flight": world,
                       "cfg_evaluation": "one batch-2 forward [cond | uncond]" if den.batched else "two batch-1 forwards",
-                      "l2": "2.8 GB of weights + ~0.6 GB of activations streamed per forward (> 126 MB L2)"},
+                      "l2": "2.8 GB of weights + ~0.6 GB of activations streamed per forward (> 50 MB L2)"},
            "latent": list(UNET_LATENT), "guide_scale": 9.0, "gpu_launches": launches,
            "achieved_tflops_per_gpu": tfs, "frac_of_bf16_peak": tfs / tf_peak, "finite": finite,
            "algorithmic_tflop_per_step": 2 * UNET_TFLOP_PER_FORWARD}
@@ -524,14 +540,15 @@ def bench_unet(device, tf_peak, peak_kind, steps=10, rank=0, world=1, with_cpu=T
     return out
 
 
-VIDEO_CLIPS, VIDEO_FRAMES, VIDEO_TEXT, VIDEO_NEW = 64, 8, 64, 32
+# 32 clips: the KV cache of 32 x 2145 positions (36 GB) + the 13.5 GB of weights fit one 80 GB H100
+VIDEO_CLIPS, VIDEO_FRAMES, VIDEO_TEXT, VIDEO_NEW = 32, 8, 64, 32
 
 
-def bench_video(device, rank, world, steps=2):
-    """BASELINE.json configs[2]: 8-frame 224x224 clips -> LanguageBind video tower (temporal attention) + projector +
-    Vicuna-7B prefill over 8 x 256 vision + 65 text tokens + 32 greedy tokens, data-parallel batch 64 over N GPUs: the 64
-    clips are SHARDED 64/N per rank (strong scaling), inputs start in pinned host memory (H2D inside the timed region), one
-    NCCL all_gather of the generated ids. value = 64 clips / max-over-ranks step time."""
+def bench_video(device, rank, world, steps=2, outputs=None):
+    """BASELINE.json configs[2] at a global batch of VIDEO_CLIPS: 8-frame 224x224 clips -> LanguageBind video tower (temporal
+    attention) + projector + Vicuna-7B prefill over 8 x 256 vision + 65 text tokens + 32 greedy tokens, data-parallel over N
+    GPUs: the clips are SHARDED VIDEO_CLIPS/N per rank (strong scaling), inputs start in pinned host memory (H2D inside the
+    timed region), one NCCL all_gather of the generated ids. value = VIDEO_CLIPS clips / max-over-ranks step time."""
     from vitron_b200 import ops, param_shapes as PS
     from vitron_b200.dist import gather_results, shard_range
     from vitron_b200.vision_tower import VisionConfig
@@ -561,7 +578,10 @@ def bench_video(device, rank, world, steps=2):
         new = out[:, -VIDEO_NEW:].contiguous()
         if world > 1:
             new = gather_results(new, VIDEO_CLIPS)
-        return new.cpu()
+        new = new.cpu()
+        if outputs is not None:
+            outputs["video_tokens"] = new
+        return new
     step()
     if world > 1:
         dist.barrier()
@@ -573,10 +593,10 @@ def bench_video(device, rank, world, steps=2):
         dist.barrier()
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t)
-    out = {"metric": "video clips/s: 8-frame LanguageBind video tower + Vicuna-7B prefill (2113 tokens) + 32 greedy tokens, global batch 64",
+    out = {"metric": f"video clips/s: 8-frame LanguageBind video tower + Vicuna-7B prefill (2113 tokens) + 32 greedy tokens, global batch {VIDEO_CLIPS}",
            "value": VIDEO_CLIPS / (ms * 1e-3), "unit": "clips/s", "n_gpus": world, "steps": steps, "warmup": 1, "ms_per_step": ms,
            "higher_is_better": True, "scaling": "strong", "dtype": "bf16", "data": "synthetic",
-           "config": {"workload": "BASELINE.json configs[2]: 64 clips sharded 64/N per GPU", "clips_per_gpu": clips, "frames": T,
+           "config": {"workload": f"BASELINE.json configs[2] at {VIDEO_CLIPS} clips, sharded {VIDEO_CLIPS}/N per GPU", "clips_per_gpu": clips, "frames": T,
                       "prompt_tokens": S, "new_tokens": VIDEO_NEW, "parallelism": f"dp{world}"},
            "generated_tokens_per_s": VIDEO_CLIPS * VIDEO_NEW / (ms * 1e-3), "gpu_launches": launches,
            "h2d_bytes_per_step": clips * 3 * T * 224 * 224 * 4 + ids.numel() * 8, "d2h_bytes_per_step": VIDEO_CLIPS * VIDEO_NEW * 8}
@@ -591,7 +611,7 @@ def run_ours(args, rank, world):
     device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(device)
     if not lib.vb200_device_ok():
-        raise RuntimeError("vitron_b200 needs an sm_100 (B200) device")
+        raise RuntimeError("vitron_b200 needs an sm_90 (H100) device")
     dist = None
     if world > 1:
         import torch.distributed as dist
@@ -609,8 +629,11 @@ def run_ours(args, rank, world):
             return gather_results(new.contiguous(), world * BATCH)
         return new
 
+    outputs = {}   # what the timed path returned in its last step (--dump-outputs)
+
     def step_resident():
-        return step(pixels_d, ids_d)
+        outputs["tokens"] = step(pixels_d, ids_d)
+        return outputs["tokens"]
 
     # e2e starts from what the reference's caller holds: decoded uint8 336x336 RGB images (BASELINE.json configs[1]) in
     # pinned host memory. They cross PCIe as uint8 and the LanguageBind transform (resize 224 bicubic, crop, normalise —
@@ -627,7 +650,8 @@ def run_ours(args, rank, world):
         else:
             px = pixels_pin.to(device, non_blocking=True)
         ids = ids_pin.to(device, non_blocking=True)
-        return step(px, ids).cpu()
+        outputs["e2e_tokens"] = step(px, ids).cpu()
+        return outputs["e2e_tokens"]
 
     for _ in range(max(args.warmup, 3)):
         step_resident()
@@ -638,10 +662,12 @@ def run_ours(args, rank, world):
     l0 = ops.launch_count()
     ms = timed(step_resident, args.steps)
     launches = (ops.launch_count() - l0) // args.steps
+    dumped = {"tokens": outputs["tokens"]}
     if world > 1:
         dist.barrier()
     step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
+    dumped["e2e_tokens"] = outputs["e2e_tokens"]
     sampler.stop_flag = True
     sampler.join(timeout=2)
     t = torch.tensor([ms, ms_e2e], device=device, dtype=torch.float64)
@@ -703,20 +729,22 @@ def run_ours(args, rank, world):
         del model
         model = None
         torch.cuda.empty_cache()
-        video_line = bench_video(device, rank, world)
+        video_line = bench_video(device, rank, world, steps=args.steps, outputs=dumped)
     # ---- the UNet half of the metric (every rank takes part when N > 1)
     unet_line = None
     if not args.no_unet:
         del model
         torch.cuda.empty_cache()
         _, tf_peak_all, kind_all = measured_peaks()
-        unet_line = bench_unet(device, tf_peak_all, kind_all, steps=max(10, args.steps), rank=rank, world=world,
-                               with_cpu=(rank == 0))
+        unet_line = bench_unet(device, tf_peak_all, kind_all, steps=args.steps, rank=rank, world=world,
+                               with_cpu=(rank == 0), outputs=dumped)
     if rank == 0:
         if video_line is not None:
             line["video_cfg2"] = video_line
         if unet_line is not None:
             line["unet"] = unet_line
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumped)
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.barrier()
@@ -727,13 +755,15 @@ def run_ours(args, rank, world):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps of every leg")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--e2e-input", default="raw", choices=["raw", "processed"],
                     help="e2e arm input: raw uint8 336x336 images (device-side transform) or pre-processed fp32 pixels")
     ap.add_argument("--no-unet", action="store_true", help="skip the i2vgen-xl UNet3D steps/s measurement")
     ap.add_argument("--no-video", action="store_true", help="skip the configs[2] video batch-64 measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's results (token ids, UNet latent) as DIR/<name>.npy")
     ap.add_argument("--profile", action="store_true",
                     help="ncu launch-list mode: one un-graphed step with 4 decode tokens, no timing loops")
     args = ap.parse_args()

@@ -1,4 +1,4 @@
-/* vitron_b200 — C ABI of the B200 (sm_100a) kernels behind Vitron's multimodal forward path.
+/* vitron_b200 — C ABI of the H100 (sm_90a) kernels behind Vitron's multimodal forward path.
  *
  * The reference (SkyworkAI/Vitron) has no FFI of its own: its "operator interface" for this path
  * is a set of torch nn.Module forwards (SURVEY.md §8b).  Every entry point below replaces the
@@ -57,7 +57,7 @@ typedef struct vb_epilogue {
 /* ---- library ---------------------------------------------------------------------------- */
 const char* vb200_version(void);
 const char* vb200_last_error(void); /* text of the last CUDA error seen by this library */
-int vb200_device_ok(void);          /* 1 iff the current device is sm_100 (B200) */
+int vb200_device_ok(void);          /* 1 iff the current device is sm_90 (H100) */
 /* Programmatic Dependent Launch for the decode-step kernels (gemv, decode attention, splice, rope table,
  * arg-max): when on, each of them is launched with programmaticStreamSerialization and overlaps its
  * prologue / weight prefetch with the tail of its predecessor. Returns the previous setting.
@@ -65,25 +65,25 @@ int vb200_device_ok(void);          /* 1 iff the current device is sm_100 (B200)
  * first weight groups BEFORE the dependency wait) must be a constant, i.e. not written by kernels still in flight on the
  * stream; activations used as W (attention-style products) belong on the M > 16 paths or in a PDL-off region. */
 int vb200_set_pdl(int enable);
-/* Attention kernel selection for vb200_attention: 0 = automatic (tcgen05/TMEM kernel for unmasked head_dim
- * 64/128 with >= 96 query rows, mma.sync otherwise), 1 = mma.sync only, 2 = tcgen05 whenever supported.
+/* Attention kernel selection for vb200_attention: 0 = automatic (wgmma kernel for head_dim 40..160
+ * with >= 96 query rows, mma.sync otherwise), 1 = mma.sync only, 2 = wgmma whenever supported.
  * Both kernels compute the same function; the switch exists so the parity tests can pin each of them. */
 int vb200_set_attention_impl(int impl);
-/* Diagnostics for the tcgen05 attention kernel: every mbarrier wait in it is bounded (~0.5 s); if one expires
+/* Diagnostics for the wgmma attention kernel: every mbarrier wait in it is bounded (~0.5 s); if one expires
  * the CTA drains instead of hanging the GPU and records where. out3 = {site id (0 = never fired), packed block
  * index, thread}; reading clears the record. Synchronises the device. */
 int vb200_attention_watchdog(uint32_t* out3);
-/* Resident CTAs per SM (registers / shared memory) of the tcgen05 attention kernel for head_dim 64 or 128. */
+/* Resident CTAs per SM (registers / shared memory) of the wgmma attention kernel for head_dim 64 or 128. */
 int vb200_attention_tc_occupancy(int head_dim);
 
-/* ---- GEMM: out[M,N] = epi(A[M,K] @ W[N,K]^T), tcgen05 + TMA (gemm_tcgen05.cu) --------------
+/* ---- GEMM: out[M,N] = epi(A[M,K] @ W[N,K]^T), wgmma + TMA (gemm.cu, gemm_v2.cuh) -------
  * Replaces every nn.Linear on the path: HF LlamaAttention/LlamaMLP/lm_head (transformers 4.31,
  * call sites vitron/model/language_model/llava_llama.py:91-102), CLIPAttention/CLIPMLP
  * (languagebind/image/modeling_image.py:136-151), mm_projector (multimodal_projector/
  * builder.py:33-51), region MLP (region_extractor/layer.py:17-20), UNet/SEEM/GLIGEN linears.
- * M <= 16 runs the weight-streaming kernel (gemv.cu: HBM-bound, no workspace). 16 < M <= 64 runs swap-AB + split-K (weights stream through the 128-row MMA slot; the CTA that completes
- * a tile last reduces the partials in split order and applies the epilogue) and needs the workspace
- * reported by vb200_gemm_bf16_workspace_size, zero-filled once by the caller before its first use. lda/ldw/ldo in elements, multiples of 8. */
+ * M <= 16 runs the weight-streaming kernel (gemv.cu: HBM-bound, no workspace). 16 < M <= 64 with a large weight runs swap-AB + split-K (weights stream through the 128-row tile slot; a reduce
+ * kernel sums the partials in split order and applies the epilogue) and needs the workspace reported by
+ * vb200_gemm_bf16_workspace_size; so do the split-K shapes of M > 64 (else the call runs unsplit). lda/ldw/ldo in elements, multiples of 8. */
 size_t vb200_gemm_bf16_workspace_size(int64_t M, int64_t N, int64_t K);
 int vb200_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void* out, int64_t ldo,
                     int64_t M, int64_t N, int64_t K, const vb_epilogue* epi, void* workspace,
@@ -91,27 +91,26 @@ int vb200_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void
 
 
 
-/* ---- implicit-GEMM convolution on NHWC activations, im2col-free (gemm_tcgen05.cu) ----------
+/* ---- implicit-GEMM convolution on NHWC activations, im2col-free (gemm.cu) ----------------
  * X [nb,h,w,cin]; Wt [cout, kh*kw, ceil64(cin)] (zero padded); out [nb,ho,wo,cout].
  * Replaces nn.Conv2d 3x3/1x1 (i2vgen util.py:651,677; Upsample/Downsample util.py:579-607,
  * 732-756), Conv3d (3,1,1) as kh=3,kw=1 over [b, f, h*w, c] (util.py:1360-1375), SEEM FPN convs
  * (transformer_encoder_fpn.py:54-107). stride in {1,2}. Convolutions whose output-pixel tiles cannot fill the SMs
- * (the 1280-channel UNet levels) run split-K over (tap, channel-chunk) steps: fp32 partials + tile counters in the
- * workspace reported by vb200_conv_nhwc_workspace_size (0 for every other shape), zero-filled ONCE by the caller
- * and left zeroed; with workspace == NULL the call runs unsplit. */
+ * (the 1280-channel UNet levels) run split-K over (tap, channel-chunk) steps: fp32 partials in the
+ * workspace reported by vb200_conv_nhwc_workspace_size (0 for every other shape); with workspace == NULL the call
+ * runs unsplit. */
 size_t vb200_conv_nhwc_workspace_size(int64_t nb, int64_t h, int64_t w, int64_t cin, int64_t cout, int kh, int kw,
                                       int stride, int pad_h, int pad_w);
 int vb200_conv_nhwc_bf16(const void* X, const void* Wt, void* out, int64_t nb, int64_t h,
                          int64_t w, int64_t cin, int64_t cout, int kh, int kw, int stride,
                          int pad_h, int pad_w, const vb_epilogue* epi, void* workspace,
                          size_t workspace_bytes, cudaStream_t stream);
-/* 0 = the compile-time-specialised kernel (gemm_v2) whenever the operands allow its 256-bit epilogue accesses
- * (default), 1 = the generic kernel only. Returns the previous setting. For A/B measurements and parity tests. */
+/* 0 = epilogue variants specialised by feature set (default), 1 = only the variants that resolve every epilogue
+ * feature at run time. Returns the previous setting. For A/B measurements and parity tests. */
 int vb200_set_gemm_impl(int impl);
 /* Variant switches / measurement aids of the v2 kernel. `resident_b` is a bit set (default 1): bit 0 = the "weight slab stays
- * in shared memory" variant for K <= 320, bit 1 = also for K <= 640, bit 2 = force the CTA-pair (tcgen05 cta_group::2) variant
- * wherever it applies (default: K >= 2048 only), bit 3 = never use it. `dbg`: bit 0 makes the epilogue skip its work, bit 1
- * only its global stores (wrong results: timing of the main loop / of the epilogue math alone). -1 keeps a setting.
+ * in shared memory" variant for K <= 320, bit 1 = also for K <= 640, other bits are ignored. `dbg`: bit 0 makes the
+ * epilogue store nothing (wrong results: timing of the main loop alone). -1 keeps a setting.
  * Returns the previous (resident_b | dbg << 8). */
 int vb200_set_gemm_debug(int resident_b, int dbg);
 

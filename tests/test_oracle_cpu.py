@@ -343,7 +343,7 @@ def test_gligen_autoencoder_scale_factor_matches_live_reference():
     missing = ref.load_state_dict(sd, strict=False)
     assert not missing.missing_keys, missing.missing_keys
 
-    class OracleVAE:  # the unscaled i2vgen-style interface the wrapper sits on (CPU stand-in for the B200 AutoencoderKL)
+    class OracleVAE:  # the unscaled i2vgen-style interface the wrapper sits on (CPU stand-in for the CUDA AutoencoderKL)
         def encode(self, x):
             mean, logvar, _ = V.encode_moments(sd, x, dd)
             return DiagonalGaussianDistribution(torch.cat([mean, logvar], 1))

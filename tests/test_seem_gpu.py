@@ -181,9 +181,9 @@ def test_seem_inference_mode_without_aux_outputs(cuda):
 
 
 def test_seem_interactive_prompts_vs_reference_golden(cuda):
-    """Grounding / audio token prompts, spatial point prompts and the refimg -> visual route on the B200 kernels against the
+    """Grounding / audio token prompts, spatial point prompts and the refimg -> visual route on the CUDA kernels against the
     golden outputs of the UNMODIFIED reference decoder (tests/golden/seem_prompts_tiny.pt): the self-attention over
-    [object queries | prompt tokens] runs as masked attention on the tcgen05 kernel."""
+    [object queries | prompt tokens] runs as masked attention on the wgmma kernel."""
     import os
     from oracle.weights import seeded_state_dict
     from vitron_b200.seem import MultiScaleMaskedTransformerDecoder

@@ -165,3 +165,32 @@ def test_midsize_vs_oracle(cuda):
     got = m.generate(ids.to(cuda), attention_mask=am.to(cuda), images=[i.to(cuda) for i in imgs], regions=regions,
                      do_sample=False, max_new_tokens=6, eos_token_id=eos, pad_token_id=0)
     assert int(got[0, L]) == eos and (got[0, L + 1:] == 0).all()
+
+
+@pytest.mark.parametrize("B", [17, 32])
+def test_graphed_decode_with_pdl_is_reproducible(cuda, B):
+    """Batch 17..64 decode (GEMM path, not the M <= 16 GEMV) replayed from CUDA graphs with programmatic dependent launch:
+    two runs from the same prompt must generate identical tokens. Vicuna-7B layer shapes at reduced depth, video-leg
+    context length (2145 prompt positions)."""
+    from vitron_b200 import ops, param_shapes as PS
+    from vitron_b200.llama import LlamaEngine
+    from vitron_b200.vitron_model import VitronConfig
+    cfg = dict(hidden_size=4096, intermediate_size=11008, num_hidden_layers=4, num_attention_heads=32, vocab_size=32000,
+               rms_norm_eps=1e-5, rope_theta=10000.0)
+    S, NEW = 2145, 16
+    eng = LlamaEngine(cfg, cuda, max_batch=B, max_seq_len=S + NEW)
+    assert eng.use_pdl
+    sd = PS.random_state_dict(PS.vitron_shapes(VitronConfig(llm=cfg, vision=None, video=None, tokenizer_model_max_length=4096)),
+                              cuda, seed=0)
+    eng.load_state_dict({k: v for k, v in sd.items() if k.startswith("model.") or k.startswith("lm_head")})
+    del sd
+    g = torch.Generator(device=cuda).manual_seed(5)
+    emb = (torch.randn((B, S, 4096), generator=g, device=cuda) * 0.02).to(torch.bfloat16)
+    runs = []
+    with torch.no_grad():
+        for _ in range(2):
+            eng.start_decode(ops.argmax_rows(eng.prefill(emb)).long(), NEW)
+            eng.decode_steps(B, NEW - 1)
+            torch.cuda.synchronize()
+            runs.append(eng.token_log[:B, :NEW].clone())
+    assert torch.equal(runs[0], runs[1]), f"rows differing: {(runs[0] != runs[1]).any(1).nonzero().flatten().tolist()}"

@@ -1,5 +1,5 @@
 """GPU: GLIGEN's sampling chain (grounded_generation_box sampler call + decode, task_grounded_generation.py:241-263) through
-vitron_b200.gligen_sampler.grounded_sample — PLMS with the scheduled gate over the B200 UNetModel, AutoencoderKL decode —
+vitron_b200.gligen_sampler.grounded_sample — PLMS with the scheduled gate over the CUDA UNetModel, AutoencoderKL decode —
 against the same chain built from the CPU oracles (the sampler arithmetic itself is pinned against the unmodified reference
 PLMSSampler on the CPU: tests/test_oracle_cpu.py::test_gligen_plms_sampler_matches_reference_sampler). Tiny widths, 5 steps,
 mild guidance; <= 10 % inf / 8 % L2 on the decoded images."""

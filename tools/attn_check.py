@@ -1,4 +1,4 @@
-"""Quick GPU check of the tcgen05 attention kernel against fp32 eager attention + timing vs mma.sync / SDPA."""
+"""Quick GPU check of the wgmma attention kernel against fp32 eager attention + timing vs mma.sync / SDPA."""
 import math, sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

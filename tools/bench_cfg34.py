@@ -1,4 +1,4 @@
-"""Measurements for BASELINE.json configs[2] and configs[3] (SURVEY.md §8d rows 3 and 4) on one B200:
+"""Measurements for BASELINE.json configs[2] and configs[3] (SURVEY.md §8d rows 3 and 4) on one GPU:
 
 cfg3  8-frame 224x224 clips -> LanguageBind video tower (temporal attention over 8 frames) + projector +
       Vicuna-7B prefill over 8 x 256 vision + 65 text tokens + 32 greedy tokens. One GPU's share of the

@@ -1,4 +1,4 @@
-"""Measurements for SURVEY.md §8(f1): SEEM's FocalNet-L backbone (seem_focall_lang.yaml:29-47) on one B200.
+"""Measurements for SURVEY.md §8(f1): SEEM's FocalNet-L backbone (seem_focall_lang.yaml:29-47) on one GPU.
 
   * whole backbone at 1024x1024 (the BASELINE.json configs[3] image): ms / image with a pinned host image (H2D
     inside the timed region), achieved TFLOP/s on the algorithmic GEMM FLOPs;
@@ -75,7 +75,7 @@ def main():
         peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6490.5))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))   # H100 SXM data sheet unless MEASURED_PEAKS.json says otherwise
     with torch.no_grad():
         net = D2FocalNet(FOCAL_L_CFG, device=dev).load_state_dict(PS.random_state_dict(PS.focalnet_shapes(FOCAL_L), dev, seed=5))
         img = torch.randn((1, 3, a.size, a.size), generator=torch.Generator().manual_seed(1)).pin_memory()

@@ -1,4 +1,4 @@
-"""Measurement for SURVEY.md §8(f2): GLIGEN's grounded SD-1.4 UNet (openaimodel.UNetModel, gatedSA fusers) on one B200:
+"""Measurement for SURVEY.md §8(f2): GLIGEN's grounded SD-1.4 UNet (openaimodel.UNetModel, gatedSA fusers) on one GPU:
 one denoising evaluation of a 512x512 image (latent [2, 4, 64, 64]: cond + uncond rows of classifier-free guidance,
 77 text tokens, 30 grounding tokens), eager and CUDA-graph replay. Random-init weights, synthetic inputs, bf16; host
 inputs (latents + conditioning in pinned memory) and the eps prediction read back inside the timed region."""

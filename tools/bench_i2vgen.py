@@ -1,4 +1,4 @@
-"""End-to-end i2vgen-xl sample on one B200 (BASELINE.json configs[4], primary latent reading 16 x 40 x 64 = 320 x 512 px,
+"""End-to-end i2vgen-xl sample on one GPU (BASELINE.json configs[4], primary latent reading 16 x 40 x 64 = 320 x 512 px,
 50 DDIM steps, guidance 9): OpenCLIP ViT-H-14 text + image embedders -> SD-VAE encode of the conditioning image ->
 50 x (2 UNetSD_I2VGen forwards + CFG), one CUDA graph replayed per step -> SD-VAE decode of 16 frames, through
 vitron_b200.i2vgen_pipeline (the inner part of inference_i2vgen_entrance.worker, :118-209). Random-init weights of

@@ -1,5 +1,5 @@
 """Measurement for SURVEY.md §8(f2): i2vgen-xl first-stage AutoencoderKL (SD-VAE, tools/modules/config.py:110-127) on
-one B200 at the BASELINE.json configs[4] primary latent: decode of 16 frames [16, 4, 40, 64] -> [16, 3, 320, 512]
+one GPU at the BASELINE.json configs[4] primary latent: decode of 16 frames [16, 4, 40, 64] -> [16, 3, 320, 512]
 (the step after the 50 DDIM steps, inference_i2vgen_entrance.py:200-209) and encode of the conditioning image
 [1, 3, 320, 512] (:172-173). Random-init weights, synthetic inputs, bf16; CUDA-event timing with host inputs / outputs."""
 import argparse, json, os, sys

@@ -1,4 +1,4 @@
-"""vitron_b200 — B200-native (sm_100a) kernels behind SkyworkAI/Vitron's multimodal forward path.
+"""vitron_b200 — H100-native (sm_90a) kernels behind SkyworkAI/Vitron's multimodal forward path.
 
 Public drop-in surface (reference names): VitronLlamaForCausalLM / LlavaLlamaForCausalLM,
 LanguageBindImageTower / LanguageBindVideoTower, build_vision_projector, build_region_extractor,

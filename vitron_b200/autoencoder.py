@@ -6,8 +6,8 @@ DiagonalGaussianDistribution (:212-253): same constructor (`ddconfig`, `embed_di
 `encode / encode_firsr_stage / decode` entry points the i2vgen entrance calls
 (tools/inferences/inference_i2vgen_entrance.py:172-173, 205-208).
 
-B200 design: NHWC bf16 end to end; every 3x3 conv (incl. stride-2 downsample and the conv after the nearest
-upsample) is the TMA implicit-GEMM tcgen05 kernel with bias / residual in the epilogue; GroupNorm(32, eps 1e-6) +
+Design: NHWC bf16 end to end; every 3x3 conv (incl. stride-2 downsample and the conv after the nearest
+upsample) is the TMA implicit-GEMM wgmma kernel with bias / residual in the epilogue; GroupNorm(32, eps 1e-6) +
 SiLU is one fused NHWC kernel; the 1x1 shortcut / q,k,v / proj_out convs are GEMMs on the pixel rows (q and k
 share one GEMM); the single-head c-channel attention (head_dim = 512, outside the flash kernels' range) is
 QK^T GEMM (fp32 scores, scale in the epilogue) -> row softmax kernel -> PV GEMM with V produced already

@@ -1,8 +1,8 @@
-"""Build the C-ABI CUDA library (libvitron_b200.so) in-tree with nvcc for sm_100a.
+"""Build the C-ABI CUDA library (libvitron_b200.so) in-tree with nvcc for sm_90a (H100).
 
 `python -m vitron_b200.build` or `vitron_b200.build.build()`.  Object files are cached by source
-mtime under vitron_b200/csrc/_obj so incremental rebuilds take seconds.  The .so is git-ignored but
-travels to the GPU box with the repo snapshot.
+mtime under vitron_b200/csrc/_obj so incremental rebuilds take seconds.  The .so and the objects are build products
+(git-ignored): a fresh checkout builds them before first use.
 """
 import os
 import subprocess
@@ -14,9 +14,9 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libvitron_b200.so")
-SOURCES = ["core.cu", "gemm_tcgen05.cu", "gemm_v2_bn256.cu", "gemm_v2_bn160.cu", "gemm_v2_bn128.cu", "gemm_v2_bn64.cu", "gemm_v2_bn32.cu", "gemm_v2_resb.cu", "gemm_v2_cl.cu", "gemv.cu", "norm.cu", "attention.cu", "attention_tc.cu", "llm.cu", "vision.cu", "focal.cu", "preprocess.cu"]
+SOURCES = ["core.cu", "gemm.cu", "gemm_v2_bn256.cu", "gemm_v2_bn160.cu", "gemm_v2_bn128.cu", "gemm_v2_bn64.cu", "gemm_v2_bn32.cu", "gemm_v2_resb.cu", "gemv.cu", "norm.cu", "attention.cu", "attention_tc.cu", "llm.cu", "vision.cu", "focal.cu", "preprocess.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC,
 ]
 
@@ -38,6 +38,7 @@ def _stale(target, deps):
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
     headers = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "gemm_common.cuh"), os.path.join(CSRC, "gemm_v2.cuh"),
+               os.path.join(CSRC, "wgmma.cuh"),
                os.path.join(ROOT, "include", "vitron_b200.h")]
     nvcc = _nvcc()
     jobs = []
@@ -59,7 +60,7 @@ def build(force=False, verbose=False):
     with ThreadPoolExecutor(max_workers=min(8, max(1, len(jobs)))) as ex:
         list(ex.map(run, jobs))
     if force or jobs or _stale(LIB, objs):
-        run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

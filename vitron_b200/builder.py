@@ -5,7 +5,7 @@
                               device_map="auto", device="cuda", **kwargs)
 
 so that `inference_image.py:19` / `inference_video.py` / `app.py` run unchanged after
-`from vitron_b200.builder import load_pretrained_model`. The model returned is the B200 drop-in
+`from vitron_b200.builder import load_pretrained_model`. The model returned is the CUDA drop-in
 (`VitronLlamaForCausalLM`), the processors are the device-side LanguageBind transforms.
 
 What the reference's loader does through `transformers` / `peft`, restated on plain files (neither library is needed to
@@ -18,7 +18,7 @@ read a checkpoint directory):
   * special tokens added to the tokenizer and the embeddings resized (builder.py:139-146);
   * 8-bit / 4-bit loading (bitsandbytes, :36-46) is not offered: the path computes in bf16 — a request raises ValueError.
 `cache_dir`, `device_map`, `torch_dtype` keywords are accepted and ignored like any other `from_pretrained` keyword the
-B200 path has no use for. Extra keywords: `tokenizer=` (a ready tokenizer object instead of `AutoTokenizer.from_pretrained`),
+CUDA path has no use for. Extra keywords: `tokenizer=` (a ready tokenizer object instead of `AutoTokenizer.from_pretrained`),
 `max_batch=` / `max_seq_len=` (KV-cache capacity of the engine; default 8 x context_len)."""
 import glob
 import json

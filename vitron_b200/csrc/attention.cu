@@ -2,7 +2,7 @@
 //
 // flash_attn_kernel: 64 query rows per CTA (4 warps x 16 rows), 64-key blocks streamed through a
 // 2-stage cp.async ring, online softmax in fp32 registers, bf16 tensor-core MMAs
-// (mma.sync m16n8k16; the tcgen05/TMEM version of this kernel is the round-2 item in DESIGN.md).
+// (mma.sync m16n8k16; the wgmma version of this kernel is attention_tc.cu).
 // Generic element strides let it read q/k/v in place from fused QKV GEMM outputs.
 //
 // Replaces: HF LlamaAttention eager path (prefill; restated in vitron/train/
@@ -462,7 +462,7 @@ int vb_attention_tc(const void* q, const void* k, const void* v, void* out, int6
                     int64_t m_sh, int64_t m_sq, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t vb_attention_tc_workspace(int64_t B, int64_t H, int64_t Sq, int64_t Skv, int64_t head_dim, int causal);
 
-static int g_attention_impl = 0;  // 0 auto, 1 mma.sync only, 2 tcgen05 whenever the shape is supported
+static int g_attention_impl = 0;  // 0 auto, 1 mma.sync only, 2 wgmma whenever the shape is supported
 extern "C" int vb200_set_attention_impl(int impl) {
   VB_CHECK_ARG(impl >= 0 && impl <= 2);
   g_attention_impl = impl;
@@ -498,7 +498,7 @@ extern "C" int vb200_attention_ws(const void* q, const void* k, const void* v, v
   VB_CHECK_ARG(H <= 65535 && B <= 65535);
   const int64_t strides[12] = {q_sb, q_ss, q_sh, k_sb, k_ss, k_sh, v_sb, v_ss, v_sh, o_sb, o_ss, o_sh};
   for (int i = 0; i < 12; ++i) VB_CHECK_ARG(strides[i] % 8 == 0);
-  // tcgen05 / TMEM kernel (attention_tc.cu): head_dim 64 / 128 natively, 40 / 80 / 160 zero-padded by the TMA unit,
+  // wgmma kernel (attention_tc.cu): head_dim 64 / 128 natively, 40 / 80 / 160 zero-padded by the TMA unit,
   // boolean masks applied in registers; taken whenever the query rows fill most of a 128-row tile. Short queries and
   // operand layouts a tensor map cannot describe stay on the mma.sync kernel below.
   if (g_attention_impl != 1 && Skv >= 1 && (Sq >= 96 || g_attention_impl == 2)) {

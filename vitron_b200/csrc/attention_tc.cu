@@ -1,4 +1,4 @@
-// vitron_b200 — flash attention on tcgen05 tensor cores with TMEM accumulators (sm_100a).
+// vitron_b200 — flash attention on sm_90a warpgroup MMA (wgmma), operands fed by TMA through mbarriers.
 //
 //   O = softmax(Q K^T * scale [causal, kv_len, bool mask]) V     bf16 in / out, fp32 math
 //   head_dim 64 / 128 natively; 40 / 80 / 160 (GLIGEN, attention.py:192-257) run the 64 / 128 / 192-column
@@ -8,27 +8,25 @@
 //   out, applied to S in registers; a row with every key masked yields zeros.
 //
 // One CTA = 128 query rows of one (batch, head); keys stream through in blocks of 64.
-//   warp 0      TMA producer: Q once, K_j / V_j into 2-stage 128B-swizzled rings (4-D tensor maps over the
-//               caller's strided [B, S, H, D] views, so fused QKV buffers are read in place)
-//   warp 1      MMA issuer:   S_j = Q K_j^T  (M128 x N64 x K=D, both K-major)   -> TMEM S[j&1]
-//                             O  += P_j V_j  (M128 x N=D x K64, V is MN-major)   -> TMEM O
-//               QK_{j+1} is issued BEFORE PV_j, so the tensor pipe works on PV_j while the softmax warps
-//               are already on block j+1 (S is double buffered in TMEM).
-//   warps 2..5  softmax: thread == query row (tcgen05.ld 32x32b), so row max / sum need no shuffles;
-//               P_j goes to smem (bf16, K-major, swizzled) as the A operand of PV_j; O stays in TMEM and is
-//               rescaled lazily (only when the running max grows by more than 2^8), final 1/l in the epilogue.
-// Two CTAs fit per SM (TMEM 256 columns, <= 113 KB smem each) so one CTA's softmax overlaps the other's MMAs.
+//   warpgroup 0      TMA producer (one thread): Q once, K_j / V_j into 2-stage 128B-swizzled rings (4-D tensor maps
+//                    over the caller's strided [B, S, H, D] views, so fused QKV buffers are read in place)
+//   warpgroups 1, 2  query rows [64 (wg - 1), +64): S_j = Q K_j^T (wgmma m64 n64, both operands K-major in shared
+//                    memory) into registers, online softmax in registers (a row lives in the 4 threads of a quad), then
+//                    O += P_j V_j with P_j as the register A operand (the S accumulator fragment IS the A fragment
+//                    layout, so P never touches shared memory) and V_j read MN-major (transposed B descriptor).
+// setmaxnreg hands the producer's registers to the consumers (O of a 64 x 192 tile is 96 fp32 per thread).
 //
 // Replaces (when there is no boolean mask and D in {64, 128}) the mma.sync kernel of attention.cu for:
 // LLaMA prefill, CLIP ViT, UNet spatial self/cross attention, SEEM pixel-decoder encoder, SEEM self-attn.
 #include "common.cuh"
 #include "vitron_b200.h"
+#include "wgmma.cuh"
 
 namespace vb {
 
 constexpr int TC_BM = 128;  // query rows per CTA
 constexpr int TC_BN = 64;   // keys per block
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 384;  // producer warpgroup + two consumer warpgroups
 
 struct TcAttnParams {
   bf16* o;
@@ -57,7 +55,7 @@ __device__ __forceinline__ unsigned long long gtime_ns() {
   return t;
 }
 
-__device__ __noinline__ void tc_wait_slow(uint64_t* bar, uint32_t parity, volatile uint32_t* abort_flag, int site) {
+__device__ __forceinline__ void tc_wait_slow(uint64_t* bar, uint32_t parity, volatile uint32_t* abort_flag, int site) {
   const unsigned long long t0 = gtime_ns();
   while (!mbar_try_wait(bar, parity)) {
     if (*abort_flag) return;
@@ -80,72 +78,44 @@ __device__ __forceinline__ void tc_wait(uint64_t* bar, uint32_t parity, volatile
   tc_wait_slow(bar, parity, abort_flag, site);
 }
 
-// MN-major operand (rows = K index, 128-byte rows of 64 MN elements, 128B swizzle):
-// SBO = stride between groups of 8 K rows, LBO = stride between 64-element MN atoms.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
 __device__ __forceinline__ float ex2_approx(float x) {  // MUFU.EX2, flush-to-zero: exp2(-inf) = 0, no denormal fix-up
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
+template <int HD>
+constexpr int tc_smem_bytes() {
+  return TC_BM * HD * 2 + 4 * TC_BN * HD * 2 + 128;   // Q + 2-stage K and V rings + barriers
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 template <int HD>
-__global__ void __launch_bounds__(TC_THREADS)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                      const __grid_constant__ CUtensorMap tmap_v, const TcAttnParams p) {
   pdl_trigger();
-  pdl_wait();   // (the tcgen05 / mbarrier set-up below touches no global data, but the kernel's first TMA load follows at once)
+  pdl_wait();   // (the mbarrier set-up below touches no global data, but the kernel's first TMA load follows at once)
   constexpr int KC = HD / 64;                   // 64-element chunks along the head dim
-  constexpr int Q_BYTES = TC_BM * HD * 2;       // [KC][128][64]
-  constexpr int K_BYTES = TC_BN * HD * 2;       // [KC][64][64]   K-major
-  constexpr int V_BYTES = TC_BN * HD * 2;       // [KC][64 keys][64]   MN-major atoms
-  constexpr int P_BYTES = TC_BM * TC_BN * 2;    // [128][64]   K-major
-  constexpr uint32_t TMEM_COLS = (2 * TC_BN + HD <= 128) ? 128 : (2 * TC_BN + HD <= 256) ? 256 : 512;
-  constexpr uint32_t S_COL = 0, O_COL = 2 * TC_BN;
+  constexpr int Q_BYTES = TC_BM * HD * 2;       // [KC][128 rows][64]   K-major
+  constexpr int K_BYTES = TC_BN * HD * 2;       // [KC][64 keys][64]    K-major
+  constexpr int V_BYTES = TC_BN * HD * 2;       // [KC][64 keys][64]    read MN-major by the P V product
 
   // No static shared memory in this kernel, so the dynamic window starts at the (1024-byte aligned) base of the
-  // CTA's allocation; spending another KB on manual alignment would cost the second resident CTA at HD = 128.
+  // CTA's allocation, as the 128B swizzle atoms require.
   extern __shared__ __align__(1024) uint8_t smem[];
   if (smem_u32(smem) & 1023u) __trap();
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Q_BYTES;          // 2 stages
   uint8_t* sV = sK + 2 * K_BYTES;      // 2 stages
-  uint8_t* sP = sV + 2 * V_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + P_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * V_BYTES);
   uint64_t* q_full = bars;             // 1
   uint64_t* k_full = bars + 1;         // 2
-  uint64_t* k_empty = bars + 3;        // 2
+  uint64_t* k_empty = bars + 3;        // 2 (one arrival per consumer warp: wgmma.wait_group completes per warp)
   uint64_t* v_full = bars + 5;         // 2
-  uint64_t* v_empty = bars + 7;        // 2
-  uint64_t* s_full = bars + 9;         // 2
-  uint64_t* p_full = bars + 11;        // 1 (count 4: one arrive per softmax warp)
-  uint64_t* pv_done = bars + 12;       // 1
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 13);
-  volatile uint32_t* abort_flag = tmem_slot + 1;
+  uint64_t* v_empty = bars + 7;        // 2 (one arrival per consumer warp)
+  volatile uint32_t* abort_flag = reinterpret_cast<volatile uint32_t*>(bars + 9);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int qb = blockIdx.x / p.splits, sp = blockIdx.x - qb * p.splits, h = blockIdx.y, b = blockIdx.z;
   const int q0 = qb * TC_BM;
   const int kv_len = p.kv_len ? min(p.kv_len[b], p.Skv) : p.Skv;
@@ -158,33 +128,24 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   const int jb0 = sp * per_split;
   const int nblk = max(0, min(nblk_all, jb0 + per_split) - jb0);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_q);
     prefetch_tmap(&tmap_k);
     prefetch_tmap(&tmap_v);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1);
-      mbar_init(&s_full[i], 1);
+      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 8);
+      mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 8);
     }
-    mbar_init(p_full, 4);
-    mbar_init(pv_done, 1);
     *abort_flag = 0;
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================================================== TMA producer
-    if (lane == 0 && nblk > 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid == 0 && nblk > 0) {
       mbar_arrive_expect_tx(q_full, Q_BYTES);
 #pragma unroll
       for (int c = 0; c < KC; ++c) tma_load_4d(sQ + c * (TC_BM * 128), &tmap_q, q_full, c * 64, q0, h, b);
@@ -201,242 +162,143 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
         for (int c = 0; c < KC; ++c) tma_load_4d(sV + st * V_BYTES + c * (TC_BN * 128), &tmap_v, &v_full[st], c * 64, (jb0 + j) * TC_BN, h, b);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    if (nblk > 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(TC_BM, TC_BN);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(TC_BM, HD) | (1u << 16);  // B (= V) is MN-major
-      auto issue_qk = [&](int j) {
-        const int st = j & 1;
-        tc_wait(&k_full[st], (j >> 1) & 1, abort_flag, 2);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t d_tmem = tmem_base + S_COL + st * TC_BN;
+    return;
+  }
+
+  // ===================================================== consumers: QK^T, softmax, PV, epilogue
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cwg = wg - 1;
+  const int lane = tid & 31;
+  // fragment rows of this thread: tile rows r_lo (h = 0) and r_lo + 8 (h = 1); columns 8i + cq + {0, 1}
+  const int r_lo = cwg * 64 + (tid >> 5) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  float o[HD / 2];
 #pragma unroll
-          for (int ks = 0; ks < HD / 16; ++ks) {
-            const uint32_t qa = smem_u32(sQ) + (ks / 4) * (TC_BM * 128) + (ks % 4) * 32;
-            const uint32_t ka = smem_u32(sK) + st * K_BYTES + (ks / 4) * (TC_BN * 128) + (ks % 4) * 32;
-            tc_mma_bf16(d_tmem, umma_desc_kmajor_sw128(qa), umma_desc_kmajor_sw128(ka), idesc_qk, ks > 0 ? 1u : 0u);
-          }
-          tc_commit(&k_empty[st]);
-          tc_commit(&s_full[st]);
-        }
-        __syncwarp();
-      };
-      tc_wait(q_full, 0, abort_flag, 1);
-      issue_qk(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) issue_qk(j + 1);  // S[(j+1)&1] was fully read before P_{j-1} was published
-        const int st = j & 1;
-        tc_wait(p_full, j & 1, abort_flag, 3);
-        tc_wait(&v_full[st], (j >> 1) & 1, abort_flag, 4);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t d_tmem = tmem_base + O_COL;
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};   // running row max (score units)
+  float l_part[2] = {0.f, 0.f};              // this thread's share of the row sums (quad-reduced at the end)
+  const uint8_t* mrow[2] = {nullptr, nullptr};
+  if (p.mask != nullptr) {
 #pragma unroll
-          for (int ks = 0; ks < TC_BN / 16; ++ks) {
-            const uint32_t pa = smem_u32(sP) + ks * 32;                          // K-major: +16 keys = +32 B
-            const uint32_t va = smem_u32(sV) + st * V_BYTES + ks * (16 * 128);   // MN-major: +16 key rows
-            tc_mma_bf16(d_tmem, umma_desc_kmajor_sw128(pa), umma_desc_mnmajor_sw128(va, TC_BN * 128, 1024), idesc_pv,
-                        (j > 0 || ks > 0) ? 1u : 0u);
-          }
-          tc_commit(&v_empty[st]);
-          tc_commit(pv_done);
-        }
-        __syncwarp();
-      }
+    for (int hh = 0; hh < 2; ++hh) {
+      const int qrow = q0 + r_lo + 8 * hh;
+      if (qrow < p.Sq) mrow[hh] = p.mask + b * p.m_sb + h * p.m_sh + static_cast<long long>(qrow) * p.m_sq;
     }
-  } else {
-    // ===================================================== softmax / correction / epilogue (thread = row)
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    const int qrow = q0 + r;
-    const uint32_t lane_addr = static_cast<uint32_t>(quad * 32) << 16;
-    float m_used = -INFINITY;  // the max the stored exponentials are relative to
-    float l = 0.f;
-    for (int j = 0; j < nblk; ++j) {
-      const int st = j & 1;
-      tc_wait(&s_full[st], (j >> 1) & 1, abort_flag, 7);
-      tc_fence_after();
-      const uint32_t s_addr = tmem_base + lane_addr + S_COL + st * TC_BN;
-      const int kbase = (jb0 + j) * TC_BN;
-      // CTA-uniform: does any row of this tile see a masked key in this block?
-      const bool need_mask = (kbase + TC_BN > kv_end) || (p.causal && kbase + TC_BN - 1 > q0 + causal_off);
-      // boolean mask bytes of this row / key block: fetched before the wait on the TMEM load
-      uint4 mb[4];
-      bool mvec = false;
-      const uint8_t* mrow = nullptr;
-      if (p.mask != nullptr && qrow < p.Sq) {
-        mrow = p.mask + b * p.m_sb + h * p.m_sh + static_cast<long long>(qrow) * p.m_sq + kbase;
-        mvec = kbase + TC_BN <= p.Skv && (reinterpret_cast<uintptr_t>(mrow) & 15) == 0;
-        if (mvec) {
+  }
+  if (nblk > 0) tc_wait(q_full, 0, abort_flag, 1);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (j >> 1) & 1;
+    // ---- S = Q K_j^T
+    float s[TC_BN / 2];
+    tc_wait(&k_full[st], ph, abort_flag, 2);
+    wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 4; ++i) mb[i] = __ldg(reinterpret_cast<const uint4*>(mrow) + i);
-        }
-      }
-      uint32_t sv[2][32];
-      tmem_ld_32x32(s_addr, sv[0]);
-      tmem_ld_32x32(s_addr + 32, sv[1]);
-      tmem_ld_wait();
+    for (int ks = 0; ks < HD / 16; ++ks) {
+      const uint32_t qa = smem_u32(sQ) + (ks / 4) * (TC_BM * 128) + cwg * (64 * 128) + (ks % 4) * 32;
+      const uint32_t ka = smem_u32(sK) + st * K_BYTES + (ks / 4) * (TC_BN * 128) + (ks % 4) * 32;
+      Wgmma<TC_BN>::ss(s, gmma_desc_kmajor(qa), gmma_desc_kmajor(ka), ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(s);
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+
+    // ---- masks: key range (kv_len, causal) and the boolean mask
+    const int kbase = (jb0 + j) * TC_BN;
+    const bool need_mask = (kbase + TC_BN > kv_end) || (p.causal && kbase + TC_BN - 1 > q0 + causal_off);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int qrow = q0 + r_lo + 8 * hh;
       if (need_mask) {
         const int lim = min(kv_end, p.causal ? qrow + causal_off + 1 : kv_end) - kbase;  // keys [0, lim) are live
 #pragma unroll
-        for (int c = 0; c < 2; ++c)
+        for (int i = 0; i < TC_BN / 8; ++i)
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c * 32 + i >= lim) sv[c][i] = 0xff800000u;  // -inf
+          for (int e = 0; e < 2; ++e)
+            if (8 * i + cq + e >= lim) s[4 * i + 2 * hh + e] = -INFINITY;
       }
-      if (mrow != nullptr) {
-        if (mvec) {
+      if (mrow[hh] != nullptr) {
 #pragma unroll
-          for (int w = 0; w < 16; ++w) {
-            const uint32_t word = w % 4 == 0 ? mb[w / 4].x : w % 4 == 1 ? mb[w / 4].y : w % 4 == 2 ? mb[w / 4].z : mb[w / 4].w;
+        for (int i = 0; i < TC_BN / 8; ++i)
 #pragma unroll
-            for (int bt = 0; bt < 4; ++bt)
-              if ((word >> (8 * bt)) & 0xffu) sv[(w * 4 + bt) / 32][(w * 4 + bt) % 32] = 0xff800000u;
+          for (int e = 0; e < 2; ++e) {
+            const int kk = kbase + 8 * i + cq + e;
+            if (kk < p.Skv && mrow[hh][kk]) s[4 * i + 2 * hh + e] = -INFINITY;
           }
-        } else {
-#pragma unroll
-          for (int c = 0; c < 2; ++c)
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (kbase + c * 32 + i < p.Skv && mrow[c * 32 + i]) sv[c][i] = 0xff800000u;
-        }
       }
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};  // independent chains: the softmax warps are
-#pragma unroll                                                      // latency-, not issue-bound
-      for (int c = 0; c < 2; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          mx[0] = fmaxf(mx[0], __uint_as_float(sv[c][i]));
-          mx[1] = fmaxf(mx[1], __uint_as_float(sv[c][i + 1]));
-          mx[2] = fmaxf(mx[2], __uint_as_float(sv[c][i + 2]));
-          mx[3] = fmaxf(mx[3], __uint_as_float(sv[c][i + 3]));
-        }
-      const float mblk = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      // lazy rescale: keep m_used unless the running max grew by more than 2^8 in the exp2 domain
-      float corr = 1.f;
-      bool rescale = false;
-      if (mblk > m_used) {
-        if (m_used == -INFINITY) {
-          m_used = mblk;
-        } else if ((mblk - m_used) * p.scale_log2 > 8.f) {
-          corr = ex2_approx((m_used - mblk) * p.scale_log2);
-          m_used = mblk;
-          rescale = true;
-        }
-      }
-      const float moff = (m_used == -INFINITY) ? 0.f : m_used * p.scale_log2;
-      float ps[4] = {0.f, 0.f, 0.f, 0.f};
-      uint32_t pk[32];  // 64 bf16 probabilities of this row
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          const float p0 = ex2_approx(fmaf(__uint_as_float(sv[c][i]), p.scale_log2, -moff));
-          const float p1 = ex2_approx(fmaf(__uint_as_float(sv[c][i + 1]), p.scale_log2, -moff));
-          const float p2 = ex2_approx(fmaf(__uint_as_float(sv[c][i + 2]), p.scale_log2, -moff));
-          const float p3 = ex2_approx(fmaf(__uint_as_float(sv[c][i + 3]), p.scale_log2, -moff));
-          ps[0] += p0; ps[1] += p1; ps[2] += p2; ps[3] += p3;
-          pk[c * 16 + i / 2] = pack_bf16(p0, p1);
-          pk[c * 16 + i / 2 + 1] = pack_bf16(p2, p3);
-        }
-      }
-      const float psum = (ps[0] + ps[1]) + (ps[2] + ps[3]);
-      // PV_{j-1} must have retired before sP is overwritten and before O is touched
-      if (j > 0) {
-        tc_wait(pv_done, (j - 1) & 1, abort_flag, 8);
-        tc_fence_after();
-      }
-      if (__any_sync(0xffffffffu, rescale)) {  // warp-uniform TMEM traffic (aligned instructions)
-        if (j > 0) {
-#pragma unroll 1
-          for (int c = 0; c < HD; c += 32) {
-            uint32_t ov[32];
-            tmem_ld_32x32(tmem_base + lane_addr + O_COL + c, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * corr);
-            tmem_st_32x32(tmem_base + lane_addr + O_COL + c, ov);
-          }
-          tmem_st_wait();
-        }
-      }
-      l = l * corr + psum;
-      uint8_t* prow = sP + r * 128;
-#pragma unroll
-      for (int piece = 0; piece < 8; ++piece)
-        *reinterpret_cast<uint4*>(prow + ((piece ^ (r & 7)) << 4)) =
-            make_uint4(pk[piece * 4], pk[piece * 4 + 1], pk[piece * 4 + 2], pk[piece * 4 + 3]);
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
     }
-    // ---- epilogue: O / l -> bf16 -> global (row per thread)
-    if (nblk > 0) {
-      tc_wait(pv_done, (nblk - 1) & 1, abort_flag, 9);
-      tc_fence_after();
+
+    // ---- online softmax (exp2 domain), rows reduced over the 4 threads of a quad
+    uint32_t pa[TC_BN / 16][4];   // P_j as bf16 A fragments, one per 16 keys
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < TC_BN / 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * hh], s[4 * i + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[hh], mx);
+      const float corr = m_run[hh] == -INFINITY ? 1.f : ex2_approx((m_run[hh] - m_new) * p.scale_log2);
+      m_run[hh] = m_new;
+      const float moff = m_new == -INFINITY ? 0.f : m_new * p.scale_log2;
+      float ps = 0.f;
+#pragma unroll
+      for (int i = 0; i < TC_BN / 8; ++i) {
+        const float p0 = ex2_approx(fmaf(s[4 * i + 2 * hh], p.scale_log2, -moff));
+        const float p1 = ex2_approx(fmaf(s[4 * i + 2 * hh + 1], p.scale_log2, -moff));
+        ps += p0 + p1;
+        pa[i / 2][(i & 1) * 2 + hh] = pack_bf16(p0, p1);
+      }
+      l_part[hh] = l_part[hh] * corr + ps;
+#pragma unroll
+      for (int i = 0; i < HD / 8; ++i) {
+        o[4 * i + 2 * hh] *= corr;
+        o[4 * i + 2 * hh + 1] *= corr;
+      }
     }
+
+    // ---- O += P_j V_j
+    tc_wait(&v_full[st], ph, abort_flag, 4);
+    wgmma_fence_operand(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < TC_BN / 16; ++kk) {
+      const uint32_t va = smem_u32(sV) + st * V_BYTES + kk * (16 * 128);   // +16 key rows
+      Wgmma<HD>::rs_tb(o, pa[kk], gmma_desc_sw128(va, TC_BN * 128, 1024), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(o);
+    if (lane == 0) mbar_arrive(&v_empty[st]);
+  }
+
+  // ---- epilogue: O / l -> bf16 -> global (or the un-normalised partial of this key range)
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float l = l_part[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int qrow = q0 + r_lo + 8 * hh;
+    if (qrow >= p.Sq) continue;
     if (p.splits > 1) {
-      // ---- partial result of this key range: un-normalised O, the max its exponentials are relative to (exp2 domain), l
-      // (the TMEM loads are warp-aligned instructions: every lane executes them, only the stores are predicated)
-      const long long slot = ((static_cast<long long>(b) * p.H + h) * p.splits + sp) * p.Sq + min(qrow, p.Sq - 1);
-      if (qrow < p.Sq) {
-        p.ws_ml[slot * 2] = (m_used == -INFINITY) ? -INFINITY : m_used * p.scale_log2;
+      const long long slot = ((static_cast<long long>(b) * p.H + h) * p.splits + sp) * p.Sq + qrow;
+      if ((lane & 3) == 0) {
+        p.ws_ml[slot * 2] = m_run[hh] == -INFINITY ? -INFINITY : m_run[hh] * p.scale_log2;
         p.ws_ml[slot * 2 + 1] = l;
       }
       float* orow_ws = p.ws_o + slot * HD;
-#pragma unroll 1
-      for (int c = 0; c < HD; c += 32) {
-        uint32_t ov[32];
-        if (nblk > 0) {
-          tmem_ld_32x32(tmem_base + lane_addr + O_COL + c, ov);
-          tmem_ld_wait();
-        } else {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) ov[i] = 0;
-        }
-        if (qrow < p.Sq) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            if (c + i < p.D)
-              *reinterpret_cast<float4*>(orow_ws + c + i) = make_float4(__uint_as_float(ov[i]), __uint_as_float(ov[i + 1]),
-                                                                        __uint_as_float(ov[i + 2]), __uint_as_float(ov[i + 3]));
-        }
-      }
+      for (int i = 0; i < HD / 8; ++i)
+        if (8 * i + cq < p.D) *reinterpret_cast<float2*>(orow_ws + 8 * i + cq) = make_float2(o[4 * i + 2 * hh], o[4 * i + 2 * hh + 1]);
     } else {
-    const float inv = l > 0.f ? 1.f / l : 0.f;
-    bf16* orow = p.o + b * p.o_sb + h * p.o_sh + static_cast<long long>(qrow) * p.o_ss;
-#pragma unroll 1
-    for (int c = 0; c < HD; c += 32) {
-      uint32_t ov[32];
-      if (nblk > 0) {
-        tmem_ld_32x32(tmem_base + lane_addr + O_COL + c, ov);
-        tmem_ld_wait();
-      } else {
+      const float inv = l > 0.f ? 1.f / l : 0.f;
+      bf16* orow = p.o + b * p.o_sb + h * p.o_sh + static_cast<long long>(qrow) * p.o_ss;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) ov[i] = 0;
-      }
-      if (qrow < p.Sq) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 8)
-          if (c + i < p.D)
-          *reinterpret_cast<uint4*>(orow + c + i) =
-              make_uint4(pack_bf16(__uint_as_float(ov[i]) * inv, __uint_as_float(ov[i + 1]) * inv),
-                         pack_bf16(__uint_as_float(ov[i + 2]) * inv, __uint_as_float(ov[i + 3]) * inv),
-                         pack_bf16(__uint_as_float(ov[i + 4]) * inv, __uint_as_float(ov[i + 5]) * inv),
-                         pack_bf16(__uint_as_float(ov[i + 6]) * inv, __uint_as_float(ov[i + 7]) * inv));
-      }
+      for (int i = 0; i < HD / 8; ++i)
+        if (8 * i + cq < p.D)
+          *reinterpret_cast<uint32_t*>(orow + 8 * i + cq) = pack_bf16(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
     }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -507,14 +369,12 @@ static int make_qkv_map(CUtensorMap* m, const void* base, long long B, long long
 template <int HD>
 static int launch_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcAttnParams& p,
                      cudaStream_t stream) {
-  constexpr int smem = TC_BM * HD * 2 + 4 * TC_BN * HD * 2 + TC_BM * TC_BN * 2 + 128;
+  constexpr int smem = tc_smem_bytes<HD>();
   static bool attr = false;
   auto kern = flash_attn_tc_kernel<HD>;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
-    // two CTAs per SM need (nearly) the whole 228 KB at HD = 128: ask for the largest shared-memory carve-out
-    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     attr = true;
   }
   dim3 grid(((p.Sq + TC_BM - 1) / TC_BM) * p.splits, p.H, p.B);
@@ -548,16 +408,16 @@ extern "C" int vb200_attention_watchdog(uint32_t* out3) {
   return VB_OK;
 }
 
-// Resident CTAs per SM of the tcgen05 attention kernel (by registers / shared memory; TMEM allows 2).
+// Resident CTAs per SM of the wgmma attention kernel (by registers / shared memory).
 extern "C" int vb200_attention_tc_occupancy(int head_dim) {
   int n = 0;
   cudaError_t e;
   if (head_dim == 64) {
-    constexpr int smem = TC_BM * 64 * 2 + 4 * TC_BN * 64 * 2 + TC_BM * TC_BN * 2 + 128;
+    constexpr int smem = tc_smem_bytes<64>();
     cudaFuncSetAttribute(flash_attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, flash_attn_tc_kernel<64>, TC_THREADS, smem);
   } else if (head_dim == 128) {
-    constexpr int smem = TC_BM * 128 * 2 + 4 * TC_BN * 128 * 2 + TC_BM * TC_BN * 2 + 128;
+    constexpr int smem = tc_smem_bytes<128>();
     cudaFuncSetAttribute(flash_attn_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, flash_attn_tc_kernel<128>, TC_THREADS, smem);
   } else {

@@ -1,5 +1,5 @@
-// vitron_b200 — shared device helpers (sm_100a only).
-// PTX wrappers for mbarrier / TMA / tcgen05 / TMEM, plus small math helpers.
+// vitron_b200 — shared device helpers (sm_90a).
+// PTX wrappers for mbarrier / TMA, plus small math helpers (warpgroup MMA: wgmma.cuh).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -106,18 +106,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// bounded wait for the kernels whose barriers are signalled from ANOTHER CTA (cluster variants): a protocol error traps
-// after ~2 s (sticky launch error the host surfaces) instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  unsigned long long t0, t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  while (!mbar_try_wait(bar, parity)) {
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    if (t - t0 > 2000000000ull) __trap();
-  }
-}
-
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
@@ -138,42 +126,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const void* tmap, uint64_
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
       "r"(c3)
       : "memory");
-}
-
-// 2-CTA (cta_group::2) loads: issued by BOTH CTAs of a pair, each into its OWN shared memory; the complete_tx goes to the
-// mbarrier at `bar_leader` = the shared::cluster address of the LEADER CTA's barrier (mapa_rank0), which collects the bytes
-// of both CTAs before the leader issues the pair's tcgen05.mma.cta_group::2.
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const void* tmap, uint32_t bar_leader, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_leader), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const void* tmap, uint32_t bar_leader, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_leader), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// shared::cluster address of the same shared-memory location in the cluster's rank-0 CTA
-__device__ __forceinline__ uint32_t mapa_rank0(const void* smem_ptr) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(smem_u32(smem_ptr)));
-  return r;
-}
-// arrive on an mbarrier of another CTA of the cluster (address from mapa_rank0)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // TMA store smem -> global (bulk async group completion)
@@ -197,120 +149,6 @@ __device__ __forceinline__ void bulk_wait_read() {
 template <int N>
 __device__ __forceinline__ void bulk_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// tcgen05.commit: arrive on an mbarrier once all previously issued MMAs have retired.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// 2-CTA pair: arrive — once every MMA the pair has issued so far has retired — on the mbarrier at this offset in every CTA
-// of `cta_mask` (ring-slot release towards both producers, accumulator hand-over to both CTAs' epilogue warps)
-__device__ __forceinline__ void tc_commit2_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-// TMEM allocation of a CTA pair: the same warp of BOTH CTAs executes these; the columns are reserved in both SMs.
-__device__ __forceinline__ void tmem_alloc2(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs: 256 x N] (+)= A[each CTA's 128 rows] * B[each CTA's N / 2 columns]: issued by the pair's leader only.
-__device__ __forceinline__ void tc_mma2_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp receives lane (base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-        "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory descriptor, K-major operand tile stored as rows of 128 bytes with the
-// 128-byte swizzle (what a TMA box {64 bf16, rows} with CU_TENSOR_MAP_SWIZZLE_128B produces).
-// 8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major tiles.
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);       // start address
-  d |= static_cast<uint64_t>(0) << 16;                          // leading byte offset (unused)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // stride byte offset
-  d |= static_cast<uint64_t>(1) << 46;                          // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                          // SWIZZLE_128B
-  return d;
-}
-// Instruction descriptor for kind::f16 with bf16 A/B, fp32 D, both operands K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4)            // D format: f32
-         | (1u << 7)          // A format: bf16
-         | (1u << 10)         // B format: bf16
-         | ((n >> 3) << 17)   // N / 8
-         | ((m >> 4) << 24);  // M / 16
 }
 
 // ---------------------------------------------------------------- math

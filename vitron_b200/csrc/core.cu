@@ -16,7 +16,7 @@ int vb_num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-      sms = 148;
+      sms = 132;   // H100 SXM
   }
   return sms;
 }
@@ -29,11 +29,13 @@ extern "C" int vb200_set_pdl(int enable) {
   return prev;
 }
 
-extern "C" const char* vb200_version(void) { return "vitron_b200 0.1 (sm_100a)"; }
+extern "C" const char* vb200_version(void) { return "vitron_b200 0.1 (sm_90a)"; }
 extern "C" const char* vb200_last_error(void) { return g_last_error; }
 extern "C" int vb200_device_ok(void) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  int minor = 0;
+  if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+  return major == 9 && minor == 0 ? 1 : 0;   // the library holds sm_90a code only
 }

@@ -1,7 +1,7 @@
 // vitron_b200 — FocalNet backbone glue kernels (SEEM, SURVEY.md §8 f1; reference
 // modules/SEEM/demo_code/xdecoder/backbone/focal.py). All HBM / FP32-pipe bound, NHWC bf16 activations.
 //
-//   im2col_nchw        stem PatchEmbed Conv2d(3, C, k7, s4, p2) (focal.py:311-338) -> rows for the tcgen05 GEMM
+//   im2col_nchw        stem PatchEmbed Conv2d(3, C, k7, s4, p2) (focal.py:311-338) -> rows for the wgmma GEMM
 //   dwconv_gelu<K>     focal_layers[l] = depthwise Conv2d(k, groups=C, bias=False) + GELU (focal.py:80-89,105)
 //   colsum / finalize  ctx_global = GELU(mean_hw(ctx)) (focal.py:107), deterministic two-stage reduction
 //   focal_modulate     ctx_all = (sum_l ctx_l * gate_l + ctx_global * gate_L) [/ (L+1)] (focal.py:103-111)
@@ -13,7 +13,8 @@
 namespace vb {
 
 // ------------------------------------------------------------------ helpers
-// two fp32 lanes packed in one 64-bit register: FFMA2 on sm_100 (2 FMAs per issue slot)
+// two fp32 lanes packed in one 64-bit register (sm_90 has no packed FFMA2: fma2 is two FFMAs; the packing costs no
+// instructions, the register pair is used in place)
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
   unsigned long long r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -25,9 +26,8 @@ __device__ __forceinline__ float2 unpack2(unsigned long long v) {
   return r;
 }
 __device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  const float2 x = unpack2(a), y = unpack2(b), z = unpack2(c);
+  return pack2(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
 }
 // packed bf16 pair -> packed fp32 pair (element 0 in the low half)
 __device__ __forceinline__ unsigned long long bf2_to_f2(uint32_t w) {
@@ -469,7 +469,7 @@ static int launch_dwconv_pair(const void* x, int64_t ld_in, const void* wt, void
   bf16* op = reinterpret_cast<bf16*>(out);
   // 32-pixel strips re-read the fewest halo columns but need ~250 registers; they pay off only when there are
   // enough strips to fill the machine several times over and the kernel is small enough not to spill
-  const bool wide = g_dwconv_impl == 3;  // measured (profiles/r01_focalnet_dwconv_variants.jsonl): 16-pixel strips win at every k
+  const bool wide = g_dwconv_impl == 3;  // opt-in only: the 16-pixel strips are the default at every k
   if (wide) {
     dwconv_gelu_pair_kernel<K, 32><<<static_cast<unsigned>((t32 + 127) / 128), 128, 0, stream>>>(xp, ld_in, wp, op, (int)nb,
                                                                                                   (int)h, (int)w, (int)c, act);
@@ -490,9 +490,8 @@ extern "C" int vb200_dwconv_nhwc(const void* x, int64_t ld_in, const void* wt, v
   VB_CHECK_ARG(nb * h * ((w + 3) / 4) * (c / 2) < (1ll << 31) - 256);  // thread indices of every variant fit 32 bits
   VB_CHECK_ARG(nb * h * w * ld_in < (1ll << 33));
   const int g = act == VB_ACT_GELU ? 1 : 0;
-  // automatic (measured, profiles/r01_focalnet_dwconv_variants.jsonl, [256^2, 192]): k = 3 / 5 -> the 16-byte loads of the
-  // 8-channel kernel win (23 vs 26 us, 37 vs 41 us); k >= 7 is instruction-bound and the channel-pair kernel wins
-  // (59 vs 73 us, 82 vs 122 us)
+  // automatic: k = 3 / 5 are load-bound -> the 16-byte loads of the 8-channel kernel; k >= 7 is instruction-bound -> the
+  // channel-pair kernel (fewer conversions per FMA)
   if (g_dwconv_impl >= 2 || (g_dwconv_impl == 0 && k >= 7)) {
     switch (k) {
       case 3: return launch_dwconv_pair<3>(x, ld_in, wt, out, nb, h, w, c, g, stream);

@@ -1,5 +1,5 @@
-// vitron_b200 — pieces shared by the tcgen05 GEMM / implicit-GEMM convolution kernels (gemm_tcgen05.cu: the generic
-// kernel incl. swap-AB; gemm_v2*.cu: the compile-time-specialised kernel). See gemm_tcgen05.cu for the design notes.
+// vitron_b200 — pieces shared by the wgmma GEMM / implicit-GEMM convolution kernel (gemm_v2.cuh) and its host side
+// (gemm.cu: planning, split-K reduce). See gemm_v2.cuh for the design notes.
 #pragma once
 #include "common.cuh"
 #include "vitron_b200.h"
@@ -8,20 +8,8 @@ namespace vb {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int NUM_EPI_WARPS = 8;  // two per TMEM lane quadrant
-constexpr int EPI_THREADS = 32 * NUM_EPI_WARPS;
-constexpr int GEMM_THREADS = 32 * (2 + NUM_EPI_WARPS);
-
-__device__ __forceinline__ void named_bar_sync(int id, int count) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
-}
-__device__ __forceinline__ void named_bar_arrive(int id, int count) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
-}
-__device__ __forceinline__ void epi_bar_sync() {  // named barrier 1: the epilogue warps only
-  asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-}
+constexpr int WGMMA_K = 16;
+constexpr int GEMM_THREADS = 3 * 128;  // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue, 64 tile rows each
 constexpr int SMEM_LIMIT = 227 * 1024;
 
 struct GemmParams {
@@ -55,11 +43,7 @@ struct GemmParams {
   float* ws;          // split-K / swap workspace [splits, rows_c, cols_c] fp32
   long long ws_split_stride;
   long long ws_ld;
-  int c_box;          // > 0: bf16 output leaves through smem + TMA store in boxes of c_box (64 | 32) columns
-  int* counters;      // one arrival counter per output tile (zero on entry, zero again on exit)
-  int rows_c, cols_c; // extent of the output in C orientation (rows = tokens, cols = features)
-  int vec_ok;         // v2: workspace rows are 32-byte aligned (N % 8 == 0) -> 256-bit partial stores
-  int dbg;            // v2 measurement aid (vb200_set_gemm_debug): bit 0 = epilogue skips its loads / math / stores
+  int dbg;            // measurement aid (vb200_set_gemm_debug): bit 0 = the epilogue stores nothing
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {

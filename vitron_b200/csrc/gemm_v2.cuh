@@ -1,23 +1,36 @@
-// vitron_b200 — tcgen05 GEMM / implicit-GEMM convolution, compile-time-specialised kernel ("v2").
+// vitron_b200 — bf16 GEMM / implicit-GEMM convolution on sm_90a warpgroup MMA (wgmma) fed by TMA through mbarriers.
 //
-// Same main loop as gemm_tcgen05.cu (TMA producer warp -> 128B-swizzled smem ring -> one thread issuing tcgen05.mma
-// into a double-buffered TMEM accumulator). What changed is everything after the accumulator is full:
+//   D[M, N] = epilogue( A[M, K] · B[N, K]^T )        (both operands K-major, fp32 accumulate)
 //
-//   * the epilogue features are TEMPLATE flags (round 1 measured the all-runtime-branch body at 13 k SASS
-//     instructions, 168 registers, `no_instruction` stalls and ~5 us per 128 x 256 tile): a variant only contains
-//     the code of the features it was instantiated with;
-//   * no shared-memory staging, no CTA-wide barriers, no TMA store: a thread owns one accumulator row
-//     (tcgen05.ld 32x32b), so a 32-column chunk is 64 contiguous bytes of bf16 output = two 256-bit stores
-//     (STG.256: full 32-byte sectors). The eight epilogue warps never wait for each other; the next chunk's
-//     tcgen05.ld and residual loads are in flight while the current chunk is processed;
-//   * split-K for tile sets that leave most SMs idle (the 5 x 8 / 16 x 40 1280-channel UNet levels: 25 tiles): fp32
-//     partials to the workspace indexed by OUTPUT row (convolutions: output pixel), then one fully parallel
-//     reduce + epilogue kernel (splitk_reduce_kernel). A last-arriving-CTA finaliser was measured first: one CTA
-//     reading splits x 128 x 256 fp32 with only its own loads in flight made the split shapes 2-5x SLOWER.
+// One persistent kernel of three warpgroups:
+//   warpgroup 0      TMA producer (one thread): A / B k-blocks into a ring of 128B-swizzled shared-memory stages
+//   warpgroups 1, 2  consumers: tile rows [64 (wg - 1), +64) — wgmma m64 n BLOCK_N k16 straight from the ring, the
+//                    accumulators in registers, then the fused epilogue from registers to global memory
+// setmaxnreg hands the producer's registers to the consumers (a 128 x 256 tile is 128 fp32 accumulators per thread).
+// Each consumer keeps one k-block of MMAs in flight and releases a ring slot as soon as the MMAs reading it retire, so the
+// producer runs ahead into the next tile while the consumers are in their epilogue. wgmma.wait_group only covers the
+// executing warp's share of the MMA, so every consumer warp arrives on the slot's empty barrier (8 arrivals per slot).
 //
-// Reference coverage as gemm_tcgen05.cu (DESIGN.md §3).
+// The A operand comes either from a plain 2-D row-major matrix or, for convolutions, straight from the NHWC activation
+// through a 4-D tensor map: every (tap, channel-chunk) k-step is one TMA box {64 ch, TW, TH, TN} fetched at the
+// tap-shifted coordinate, out-of-bounds pixels are zero-filled by the TMA unit (= zero padding), so no im2col buffer
+// exists. A box of fewer than 128 pixels leaves stale rows in the stage: they only feed accumulator rows that are never
+// stored (tile_row_to_orow).
+//
+// Epilogue features are TEMPLATE flags (F_*): a variant only contains the code of the features it was instantiated with;
+// F_ALL / F_ALL_GLU resolve every feature at run time (the generic variants, vb200_set_gemm_impl(1)).
+// RESB ("resident B"): for small K the CTA keeps ALL k-blocks of ONE n-block of the weight matrix in shared memory and
+// walks m-tiles of that n-block only; the ring then carries A alone. Without it every 128 x BN tile re-fetches its B tile
+// from L2, which bounds the small-K UNet GEMMs (K = 320: 40 KB of B per 16 KB A k-block at BN = 160).
+// Split-K (F_WS) and swap-AB write raw fp32 partials to the workspace, indexed by OUTPUT row (convolutions: output
+// pixel); splitk_reduce_kernel (gemm.cu) sums them in split order and applies the epilogue.
+//
+// Covers (reference file:line in DESIGN.md): LLaMA q/k/v/o/gate/up/down/lm_head, CLIP ViT q/k/v/out/fc1/fc2,
+// mm_projector, region MLP, every Linear / Conv2d(3x3,1x1) / Conv3d(3,1,1) of UNetSD_I2VGen, SEEM FPN convs + mask
+// einsum, GLIGEN fuser linears.
 #pragma once
 #include "gemm_common.cuh"
+#include "wgmma.cuh"
 
 namespace vb {
 
@@ -28,27 +41,14 @@ constexpr int F_RES = 4;   // out = residual + alpha * v   (residual may be null
 constexpr int F_ACT = 8;   // activation selected at run time (p.act)
 constexpr int F_GLU = 16;  // packed SwiGLU / GEGLU selected at run time (p.glu)
 constexpr int F_F32 = 32;  // fp32 output
-constexpr int F_WS = 64;   // split-K: raw fp32 partials -> workspace, last CTA finalises
+constexpr int F_WS = 64;   // raw fp32 partials -> workspace (split-K, swap-AB), reduced by splitk_reduce_kernel
 constexpr int F_ALL = F_RS | F_RB | F_RES | F_ACT | F_F32;            // every non-GLU feature at run time
 constexpr int F_ALL_GLU = F_GLU | F_RS | F_RB | F_RES | F_F32;        // every GLU combination at run time
 
-__device__ __forceinline__ void ldg_v8(const void* p, uint32_t (&v)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(p));
-}
-// residual rows may alias the output rows (in-place "z += f(z)"): plain (coherent) loads, not .nc
-__device__ __forceinline__ void ld_v8(const void* p, uint32_t (&v)[8]) {
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(p)
-               : "memory");
-}
-__device__ __forceinline__ void st_v8(void* p, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // output row (C orientation) of accumulator row r of m-block m_blk; -1 = padding row of the tile
 __device__ __forceinline__ int tile_row_to_orow(const GemmParams& p, int m_blk, int r) {
@@ -69,54 +69,43 @@ __device__ __forceinline__ int tile_row_to_orow(const GemmParams& p, int m_blk, 
   return -1;
 }
 
-// scalar epilogue of the (at most one per row) chunk that straddles N: every feature at run time, out of line
-static __device__ __noinline__ void epi_ragged(const uint32_t* acc, int n_valid, float rs, const bf16* bias, const bf16* rb,
-                                        const bf16* res, float alpha, int act, void* out, int out_fp32) {
-  for (int j = 0; j < n_valid && j < 32; ++j) {
-    float a = __uint_as_float(acc[j]) * rs;
-    if (bias != nullptr) a += __bfloat162float(bias[j]);
-    if (rb != nullptr) a += __bfloat162float(rb[j]);
-    float o = apply_act(a, act);
-    o = res != nullptr ? __bfloat162float(res[j]) + alpha * o : alpha * o;
-    if (out_fp32) reinterpret_cast<float*>(out)[j] = o;
-    else reinterpret_cast<bf16*>(out)[j] = __float2bfloat16(o);
+// two adjacent outputs (columns oc, oc + 1; the second only when `two`) of one row: residual / alpha, then the store
+template <int F>
+__device__ __forceinline__ void epi_store2(const GemmParams& p, int orow, int oc, bool two, bool vec, float v0, float v1) {
+  if constexpr ((F & F_RES) != 0) {
+    if (p.residual != nullptr) {
+      // the residual may alias the output (in-place "z += f(z)"): plain coherent loads
+      const bf16* rp = p.residual + static_cast<size_t>(orow) * p.ldr + oc;
+      v0 = fmaf(p.alpha, v0, __bfloat162float(rp[0]));
+      if (two) v1 = fmaf(p.alpha, v1, __bfloat162float(rp[1]));
+    } else {
+      v0 *= p.alpha;
+      v1 *= p.alpha;
+    }
+  }
+  if ((F & F_F32) != 0 && p.out_fp32) {
+    float* dst = reinterpret_cast<float*>(p.out) + static_cast<size_t>(orow) * p.ldo + oc;
+    if (two && vec) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+    else { dst[0] = v0; if (two) dst[1] = v1; }
+  } else {
+    bf16* dst = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(orow) * p.ldo + oc;
+    if (two && vec) *reinterpret_cast<uint32_t*>(dst) = pack_bf16(v0, v1);
+    else { dst[0] = __float2bfloat16(v0); if (two) dst[1] = __float2bfloat16(v1); }
   }
 }
 
-// RESB ("resident B"): for small K (a few k-blocks) the CTA keeps ALL k-blocks of ONE n-block of the weight matrix in shared
-// memory for its whole life and works on m-tiles of that n-block only; the ring then carries A alone. Without it every
-// 128 x BN tile re-fetches its B tile from L2: at K = 320 the level-0 UNet GEMMs moved 184 KB per tile for 0.85 us of MMA —
-// 8.6 TB/s of L2 -> SM traffic, L2-bandwidth bound (in-situ 16.7 us for M 40960, N = K = 320 against ~4 us of MMA).
-// CL ("CTA pair", tcgen05 cta_group::2): the two CTAs of a cluster (two SMs of one TPC) compute ONE 256 x BLOCK_N tile.
-// Each CTA loads its own 128 rows of A and only HALF of the B tile (BLOCK_N / 2 weight rows); the leader CTA's single MMA
-// thread issues tcgen05.mma.cta_group::2 (M = 256), which reads A and B from both CTAs' shared memory and accumulates
-// rows 0..127 into the leader's TMEM and rows 128..255 into the peer's. Per SM and k-step the same 128 x BLOCK_N x 64 MMA
-// work now needs 16 KB + BLOCK_N x 64 B of operand traffic instead of 16 KB + BLOCK_N x 128 B (BLOCK_N = 256: 32 KB instead
-// of 48 KB) — the 1-CTA kernel is bound by the L2 -> SM operand stream, not by the tensor pipe (measured in round 2:
-// main loop alone at K = 320, N >= 960 = 0.45 us per k-step against 0.27 us of MMA).
-// Protocol: both producers wait on their OWN ring-slot barrier and issue cta_group::2 TMA loads whose bytes are counted
-// by the LEADER's full barrier (which expects both CTAs' bytes); the leader's tcgen05.commit multicasts the slot release
-// and the accumulator hand-over to both CTAs; each CTA's epilogue warps drain their own TMEM and arrive on the leader's
-// accumulator-empty barrier (2 x NUM_EPI_WARPS arrivals). TMEM is allocated / freed by warp 1 of both CTAs (cta_group::2).
-template <int BLOCK_N, int STAGES, int F, bool RESB = false, bool CL = false>
+template <int BLOCK_N, int STAGES, int F, bool RESB = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_v2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmParams p) {
   constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  constexpr int B_BYTES = (CL ? BLOCK_N / 2 : BLOCK_N) * BLOCK_K * 2;   // CTA pair: this CTA's half of the B tile
+  constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
   constexpr int STAGE_BYTES = RESB ? A_BYTES : A_BYTES + B_BYTES;
-  constexpr int ACC_STAGES = 2;
-  constexpr uint32_t TMEM_COLS = (ACC_STAGES * BLOCK_N <= 32)    ? 32
-                                 : (ACC_STAGES * BLOCK_N <= 64)  ? 64
-                                 : (ACC_STAGES * BLOCK_N <= 128) ? 128
-                                 : (ACC_STAGES * BLOCK_N <= 256) ? 256
-                                                                 : 512;
   constexpr bool WS = (F & F_WS) != 0;
   constexpr bool GLU = (F & F_GLU) != 0;
-  constexpr bool F32C = (F & F_F32) != 0;  // fp32 output POSSIBLE in this variant; p.out_fp32 decides at run time
-  constexpr int NCH = BLOCK_N / 32;       // 32-column accumulator chunks per tile
-  constexpr int OUTS = GLU ? 16 : 32;     // outputs one chunk produces
-  static_assert(BLOCK_N % 32 == 0, "v2 tiles are whole 32-column chunks");
+  constexpr int NACC = BLOCK_N / 2;       // accumulators per consumer thread (64 x BLOCK_N over 128 threads)
+  static_assert(BLOCK_N % 32 == 0, "tiles are whole 32-column GLU blocks");
+  static_assert(B_BYTES % 1024 == 0, "stages stay 1024-byte aligned (128B swizzle atoms)");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem_al = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -125,466 +114,220 @@ gemm_v2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   uint8_t* smem = smem_al + (RESB ? p.num_k_blocks * B_BYTES : 0);              // the ring
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + ACC_STAGES;
-  uint64_t* b_full = tmem_empty + ACC_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(b_full + 1);
-  // per-epilogue-warp copy of the tile's additive column vector (bias [+ rowbias when one row group covers the warp's
-  // rows]) in fp32: filled BEFORE the wait for the accumulator, read back as 16-byte broadcasts. (Loading the bias from
-  // global inside every chunk put one L2 round trip, ~700 clk, on the critical path of each of a tile's 5-8 chunks:
-  // 3.5 us per 128 x 160 tile at K = 320 against 0.85 us of MMA.)
-  float* ebias = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);  // (smem = the ring base)
+  uint64_t* b_full = empty_bar + STAGES;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int tid = threadIdx.x & 127;
 
-  // Programmatic dependent launch: this grid may be scheduled while its predecessor on the stream drains. Everything up
-  // to pdl_wait() below (barrier init, TMEM allocation, tensor-map prefetch) touches no global data; every global read AND
-  // write of the kernel comes after it. The successor is released at once: it parks at its own pdl_wait().
+  // Programmatic dependent launch: barrier set-up touches no global data; every global read and write follows pdl_wait().
   pdl_trigger();
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < ACC_STAGES; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], CL ? 2 * NUM_EPI_WARPS : NUM_EPI_WARPS);
+      mbar_init(&empty_bar[i], 8);   // one arrival per consumer warp (wgmma.wait_group completes per warp)
     }
     mbar_init(b_full, 1);
     fence_barrier_init();
   }
-  uint32_t crank = 0;
-  if constexpr (CL) {
-    cluster_sync_all();   // both CTAs' barriers exist before anything arrives on them from the other CTA
-    crank = cluster_ctarank();
-  }
-  if (warp == 1) {
-    if constexpr (CL) {
-      tmem_alloc2(tmem_slot, TMEM_COLS);
-      tmem_relinquish2();
-    } else {
-      tmem_alloc(tmem_slot, TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
 
   // work units of this CTA: (m-block, n-block, split) in grouped raster order, or — RESB — the m-blocks
   // m = blockIdx.x / n_blocks, += gridDim.x / n_blocks of the ONE n-block blockIdx.x % n_blocks (grid is a multiple of n_blocks)
-  const int total_units = RESB ? p.m_blocks : CL ? ((p.m_blocks + 1) >> 1) * p.n_blocks : p.m_blocks * p.n_blocks * p.splits;
-  const int unit_first = RESB ? static_cast<int>(blockIdx.x) / p.n_blocks : CL ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int unit_step = RESB ? static_cast<int>(gridDim.x) / p.n_blocks : CL ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int total_units = RESB ? p.m_blocks : p.m_blocks * p.n_blocks * p.splits;
+  const int unit_first = RESB ? static_cast<int>(blockIdx.x) / p.n_blocks : static_cast<int>(blockIdx.x);
+  const int unit_step = RESB ? static_cast<int>(gridDim.x) / p.n_blocks : static_cast<int>(gridDim.x);
   const int my_n_blk = RESB ? static_cast<int>(blockIdx.x) % p.n_blocks : 0;
   auto work_of = [&](int unit) {
     if constexpr (RESB) {
       TileCoord t;
       t.m_blk = unit; t.n_blk = my_n_blk; t.split = 0;
       return t;
-    } else if constexpr (CL) {
-      // grouped raster over (m-block PAIR, n-block); this CTA owns m-block 2 * pair + rank (may be one past the last
-      // m-block when their number is odd: its loads are all out of bounds = zeros, its rows are never stored)
-      TileCoord t;
-      const int mpairs = (p.m_blocks + 1) >> 1;
-      const int per_group = 8 * p.n_blocks;
-      const int group = unit / per_group;
-      const int first_m = group * 8;
-      const int gsize = min(mpairs - first_m, 8);
-      const int in_group = unit - group * per_group;
-      t.m_blk = 2 * (first_m + in_group % gsize) + static_cast<int>(crank);
-      t.n_blk = in_group / gsize;
-      t.split = 0;
-      return t;
     } else {
       return decode_work(p, unit);
     }
   };
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================================================== TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (tid == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      [[maybe_unused]] uint32_t full_bar_leader = 0;
-      if constexpr (CL) full_bar_leader = mapa_rank0(full_bar);
       if constexpr (RESB) {
         mbar_arrive_expect_tx(b_full, static_cast<uint32_t>(p.num_k_blocks) * B_BYTES);
         for (int kb = 0; kb < p.num_k_blocks; ++kb)
           tma_load_2d(sB_res + kb * B_BYTES, &tmap_b, b_full, kb * BLOCK_K, my_n_blk * BLOCK_N);
       }
       for (int unit = unit_first; unit < total_units; unit += unit_step) {
-        TileCoord t = work_of(unit);
+        const TileCoord t = work_of(unit);
         int k0, k1;
         split_range(p, t.split, k0, k1);
         int cw = 0, ch = 0, cn = 0;
         if (p.a_mode == 1) {
-          int tiw = t.m_blk % p.tiles_w;
-          int rest = t.m_blk / p.tiles_w;
-          int tih = rest % p.tiles_h;
-          int tin = rest / p.tiles_h;
+          const int tiw = t.m_blk % p.tiles_w;
+          const int rest = t.m_blk / p.tiles_w;
           cw = tiw * p.tw * p.stride - p.pad_w;
-          ch = tih * p.th * p.stride - p.pad_h;
-          cn = tin * p.tn;
+          ch = (rest % p.tiles_h) * p.th * p.stride - p.pad_h;
+          cn = (rest / p.tiles_h) * p.tn;
         }
         for (int kb = k0; kb < k1; ++kb) {
-          if constexpr (CL) mbar_wait_bounded(&empty_bar[stage], phase ^ 1);
-          else mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
-          if constexpr (CL) {
-            // the leader's barrier counts the bytes of BOTH CTAs (own A rows + own half of the B tile each)
-            if (crank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * (p.a_box_bytes + B_BYTES));
-            const uint32_t fb = full_bar_leader + stage * 8;
-            if (p.a_mode == 0) {
-              tma_load_2d_2sm(sa, &tmap_a, fb, kb * BLOCK_K, t.m_blk * BLOCK_M);
-            } else {
-              int tap = kb / p.cin_chunks;
-              int cc = kb - tap * p.cin_chunks;
-              int dy = tap / p.kw, dx = tap - dy * p.kw;
-              tma_load_4d_2sm(sa, &tmap_a, fb, cc * BLOCK_K, cw + dx, ch + dy, cn);
-            }
-            tma_load_2d_2sm(sb, &tmap_b, fb, kb * BLOCK_K, t.n_blk * BLOCK_N + static_cast<int>(crank) * (BLOCK_N / 2));
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            continue;
-          }
           mbar_arrive_expect_tx(&full_bar[stage], p.a_box_bytes + (RESB ? 0 : B_BYTES));
           if (p.a_mode == 0) {
             tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, t.m_blk * BLOCK_M);
           } else {
-            int tap = kb / p.cin_chunks;
-            int cc = kb - tap * p.cin_chunks;
-            int dy = tap / p.kw, dx = tap - dy * p.kw;
+            const int tap = kb / p.cin_chunks;
+            const int cc = kb - tap * p.cin_chunks;
+            const int dy = tap / p.kw, dx = tap - dy * p.kw;
             tma_load_4d(sa, &tmap_a, &full_bar[stage], cc * BLOCK_K, cw + dx, ch + dy, cn);
           }
-          if constexpr (!RESB) tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, t.n_blk * BLOCK_N);
+          if constexpr (!RESB) tma_load_2d(sa + A_BYTES, &tmap_b, &full_bar[stage], kb * BLOCK_K, t.n_blk * BLOCK_N);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(CL ? 2 * BLOCK_M : BLOCK_M, BLOCK_N);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    if constexpr (RESB) {
-      if (unit_first < total_units) mbar_wait(b_full, 0);
-    }
-    // CTA pair: only the leader issues MMAs (they drive the tensor cores of both SMs)
-    for (int unit = (CL && crank != 0) ? total_units : unit_first; unit < total_units; unit += unit_step) {
-      TileCoord t = work_of(unit);
-      int k0, k1;
-      split_range(p, t.split, k0, k1);
-      if constexpr (CL) mbar_wait_bounded(&tmem_empty[acc], acc_phase ^ 1);
-      else mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-      for (int kb = k0; kb < k1; ++kb) {
-        if constexpr (CL) mbar_wait_bounded(&full_bar[stage], phase);
-        else mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint32_t sb = RESB ? smem_u32(sB_res + kb * B_BYTES) : sa + A_BYTES;
-          const uint64_t da = umma_desc_kmajor_sw128(sa);
-          const uint64_t db = umma_desc_kmajor_sw128(sb);
-          if constexpr (CL) {
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              tc_mma2_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb > k0 || k > 0) ? 1u : 0u);
-            tc_commit2_mc(&empty_bar[stage], 3);                      // slot free again in both CTAs
-            if (kb == k1 - 1) tc_commit2_mc(&tmem_full[acc], 3);      // accumulator halves ready in both CTAs
-          } else {
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              tc_mma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb > k0 || k > 0) ? 1u : 0u);
-            tc_commit(&empty_bar[stage]);
-            if (kb == k1 - 1) tc_commit(&tmem_full[acc]);
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (k1 <= k0 && lane == 0) tc_commit(&tmem_full[acc]);  // degenerate (never for K > 0)
-      __syncwarp();
-      if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-    }
-  } else {
-    // ===================================================== epilogue warps (independent of each other)
-    const int quad = warp & 3;          // TMEM lane quadrant this warp may read
-    const int ehalf = (warp - 2) >> 2;  // the two warps of a quadrant take alternate 32-column chunks
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int unit = unit_first; unit < total_units; unit += unit_step) {
-      const TileCoord t = work_of(unit);
-      const int r = quad * 32 + lane;  // accumulator row owned by this thread
-      const int orow = tile_row_to_orow(p, t.m_blk, r);
-      const int col0 = t.n_blk * BLOCK_N;
-      const uint32_t taddr = tmem_base + acc * BLOCK_N + (static_cast<uint32_t>(quad * 32) << 16);
-
-      // ---- per-row operands (independent of the accumulator: set up before waiting for it)
-      float rs = 1.f;
-      const bf16* rb = nullptr;
-      const bf16* rrow = nullptr;
-      if constexpr (!WS) {
-        if constexpr ((F & F_RS) != 0) {
-          if (p.rowscale != nullptr && orow >= 0) rs = __ldg(p.rowscale + orow);
-        }
-        if constexpr ((F & F_RB) != 0) {
-          if (p.rowbias != nullptr && orow >= 0)
-            rb = p.rowbias + static_cast<size_t>(orow / p.rowbias_rows) * p.N + col0;
-        }
-        if constexpr ((F & F_RES) != 0) {
-          if (p.residual != nullptr && orow >= 0)
-            rrow = p.residual + static_cast<size_t>(orow) * p.ldr + (GLU ? col0 / 2 : col0);
-        }
-      }
-      bool rb_staged = false;
-      float* sb = ebias + (warp - 2) * BLOCK_N;
-      if constexpr (!WS) {
-        int gsel = -1;
-        if constexpr ((F & F_RB) != 0) {
-          if (p.rowbias != nullptr) {
-            const int gme = orow >= 0 ? orow / p.rowbias_rows : -1;
-            const int gmax = __reduce_max_sync(0xffffffffu, gme);
-            const int gmin = __reduce_min_sync(0xffffffffu, gme < 0 ? gmax : gme);
-            if (gmax >= 0 && gmin == gmax) { gsel = gmax; rb_staged = true; }
-          }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int c = lane; c < BLOCK_N; c += 32) {
-          float bv = 0.f;
-          if (col0 + c < p.N) {
-            if (p.bias != nullptr) bv = __bfloat162float(p.bias[col0 + c]);
-            if (gsel >= 0) bv += __bfloat162float(p.rowbias[static_cast<size_t>(gsel) * p.N + col0 + c]);
-          }
-          sb[c] = bv;
-        }
-        __syncwarp();
-      }
-      uint8_t* orow_ptr = nullptr;  // first output element of this thread's row inside the tile
-      if (orow >= 0) {
-        if constexpr (WS)
-          orow_ptr = reinterpret_cast<uint8_t*>(p.ws + static_cast<size_t>(t.split) * p.ws_split_stride +
-                                                static_cast<size_t>(orow) * p.ws_ld + col0);
-        else if (F32C && p.out_fp32)
-          orow_ptr = reinterpret_cast<uint8_t*>(reinterpret_cast<float*>(p.out) + static_cast<size_t>(orow) * p.ldo +
-                                                (GLU ? col0 / 2 : col0));
-        else
-          orow_ptr = reinterpret_cast<uint8_t*>(reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(orow) * p.ldo +
-                                                (GLU ? col0 / 2 : col0));
-      }
-
-      // residual: the first chunk's loads are issued BEFORE the wait for the accumulator (they do not depend on it), the
-      // next chunk's while the current one is processed. (A 3-deep ring issued up front was measured: no gain in the
-      // UNet, +5 % on the BN = 160 residual variant from the extra registers.)
-      constexpr int MYCH = (NCH + 1) / 2;            // chunks a warp handles at most
-      constexpr int RD = MYCH < 2 ? MYCH : 2;
-      uint32_t v[2][32];
-      uint32_t rres[RD][16];
-      auto prefetch_res = [&](int ci, uint32_t (&dst)[16]) {
-        if constexpr (!WS && (F & F_RES) != 0) {
-          if (rrow != nullptr && col0 + (ci + 1) * 32 <= p.N) {
-            uint32_t a[8];
-            ld_v8(rrow + ci * OUTS, a);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) dst[j] = a[j];
-            if constexpr (!GLU) {
-              uint32_t b[8];
-              ld_v8(rrow + ci * OUTS + 16, b);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) dst[8 + j] = b[j];
-            }
-          }
-        }
-      };
-
-      if (NCH % 2 == 0 || ehalf < NCH) prefetch_res(ehalf, rres[0]);
-      if constexpr (CL) mbar_wait_bounded(&tmem_full[acc], acc_phase);
-      else mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      if (NCH % 2 == 0 || ehalf < NCH) tmem_ld_32x32(taddr + ehalf * 32, v[0]);
-#pragma unroll
-      for (int it = 0; it < MYCH; ++it) {
-        const int ci = ehalf + 2 * it;
-        if (NCH % 2 == 0 || ci < NCH) {
-          tmem_ld_wait();
-          if (ci + 2 < NCH) {
-            tmem_ld_32x32(taddr + (ci + 2) * 32, v[(it + 1) & 1]);
-            if constexpr (RD > 1) prefetch_res(ci + 2, rres[(it + 1) % RD]);
-          }
-          uint32_t(&vv)[32] = v[it & 1];
-          uint32_t(&rr)[16] = rres[it % RD];
-          const int gc = col0 + ci * 32;  // first accumulator column of this chunk
-          if (gc < p.N && !(p.dbg & 1)) {
-            const bool full = gc + 32 <= p.N;
-            if constexpr (WS) {
-              // ---------------- raw fp32 partials
-              if (orow >= 0) {
-                float* dst = reinterpret_cast<float*>(orow_ptr) + ci * 32;
-                if (full && p.vec_ok) {
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) {
-                    const uint32_t o[8] = {vv[q * 8], vv[q * 8 + 1], vv[q * 8 + 2], vv[q * 8 + 3],
-                                           vv[q * 8 + 4], vv[q * 8 + 5], vv[q * 8 + 6], vv[q * 8 + 7]};
-                    st_v8(dst + q * 8, o);
-                  }
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j)
-                    if (gc + j < p.N) dst[j] = __uint_as_float(vv[j]);
-                }
-              }
-            } else if (full) {
-              // ---------------- fused epilogue, whole chunk, 256-bit accesses
-              float f[32];
-              {
-                const float4* sp = reinterpret_cast<const float4*>(sb + ci * 32);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 bq = sp[j];
-                  f[4 * j] = fmaf(__uint_as_float(vv[4 * j]), rs, bq.x);
-                  f[4 * j + 1] = fmaf(__uint_as_float(vv[4 * j + 1]), rs, bq.y);
-                  f[4 * j + 2] = fmaf(__uint_as_float(vv[4 * j + 2]), rs, bq.z);
-                  f[4 * j + 3] = fmaf(__uint_as_float(vv[4 * j + 3]), rs, bq.w);
-                }
-              }
-              if constexpr ((F & F_RB) != 0) {
-                if (rb != nullptr && !rb_staged) {
-                  uint32_t b0[8], b1[8];
-                  ldg_v8(rb + ci * 32, b0);
-                  ldg_v8(rb + ci * 32 + 16, b1);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) {
-                    const float2 x0 = unpack_bf16(b0[j]), x1 = unpack_bf16(b1[j]);
-                    f[2 * j] += x0.x;
-                    f[2 * j + 1] += x0.y;
-                    f[16 + 2 * j] += x1.x;
-                    f[16 + 2 * j + 1] += x1.y;
-                  }
-                }
-              }
-              if constexpr (GLU) {
-                if (p.glu == VB_GLU_SWIGLU) {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) f[j] = silu(f[j]) * f[j + 16];
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) f[j] = f[j] * gelu_erf_fast(f[j + 16]);
-                }
-              } else if constexpr ((F & F_ACT) != 0) {
-                if (p.act == VB_ACT_GELU) {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) f[j] = gelu_erf_fast(f[j]);
-                } else if (p.act == VB_ACT_SILU) {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) f[j] = silu(f[j]);
-                } else if (p.act == VB_ACT_QUICK_GELU) {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) f[j] = quick_gelu(f[j]);
-                } else if (p.act == VB_ACT_RELU) {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-                }
-              }
-              if constexpr ((F & F_RES) != 0) {
-                if (rrow != nullptr) {
-#pragma unroll
-                  for (int j = 0; j < OUTS / 2; ++j) {
-                    const float2 x = unpack_bf16(rr[j]);
-                    f[2 * j] = fmaf(p.alpha, f[2 * j], x.x);
-                    f[2 * j + 1] = fmaf(p.alpha, f[2 * j + 1], x.y);
-                  }
-                } else if (p.alpha != 1.0f) {
-#pragma unroll
-                  for (int j = 0; j < OUTS; ++j) f[j] *= p.alpha;
-                }
-              }
-              if (orow >= 0) {
-                if (F32C && p.out_fp32) {
-                  float* dst = reinterpret_cast<float*>(orow_ptr) + ci * OUTS;
-#pragma unroll
-                  for (int q = 0; q < OUTS / 8; ++q) {
-                    const uint32_t o[8] = {__float_as_uint(f[q * 8]),     __float_as_uint(f[q * 8 + 1]),
-                                           __float_as_uint(f[q * 8 + 2]), __float_as_uint(f[q * 8 + 3]),
-                                           __float_as_uint(f[q * 8 + 4]), __float_as_uint(f[q * 8 + 5]),
-                                           __float_as_uint(f[q * 8 + 6]), __float_as_uint(f[q * 8 + 7])};
-                    st_v8(dst + q * 8, o);
-                  }
-                } else {
-                  bf16* dst = reinterpret_cast<bf16*>(orow_ptr) + ci * OUTS;
-                  if (p.dbg & 2) {   // measurement aid: everything but the global stores (result kept alive through one lane)
-                    float acc_ = 0.f;
-#pragma unroll
-                    for (int j = 0; j < OUTS; ++j) acc_ += f[j];
-                    if (acc_ == 123.456f) dst[0] = __float2bfloat16(acc_);
-                  } else
-#pragma unroll
-                  for (int q = 0; q < OUTS / 16; ++q) {
-                    const uint32_t o[8] = {pack_bf16(f[q * 16], f[q * 16 + 1]),       pack_bf16(f[q * 16 + 2], f[q * 16 + 3]),
-                                           pack_bf16(f[q * 16 + 4], f[q * 16 + 5]),   pack_bf16(f[q * 16 + 6], f[q * 16 + 7]),
-                                           pack_bf16(f[q * 16 + 8], f[q * 16 + 9]),   pack_bf16(f[q * 16 + 10], f[q * 16 + 11]),
-                                           pack_bf16(f[q * 16 + 12], f[q * 16 + 13]), pack_bf16(f[q * 16 + 14], f[q * 16 + 15])};
-                    st_v8(dst + q * 16, o);
-                  }
-                }
-              }
-            } else if (orow >= 0) {
-              // ---------------- ragged last chunk of a row (N % 32 != 0; never with GLU): out-of-line scalar loop on a
-              // local copy of the accumulators (the copy keeps `v` itself in registers)
-              if constexpr (!GLU) {
-                uint32_t tmp[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) tmp[j] = vv[j];
-                epi_ragged(tmp, p.N - gc, rs, p.bias != nullptr ? p.bias + gc : nullptr, rb != nullptr ? rb + ci * 32 : nullptr,
-                           rrow != nullptr ? rrow + ci * 32 : nullptr, p.alpha, (F & F_ACT) ? p.act : VB_ACT_NONE,
-                           (F32C && p.out_fp32) ? static_cast<void*>(reinterpret_cast<float*>(orow_ptr) + ci * 32)
-                                                : static_cast<void*>(reinterpret_cast<bf16*>(orow_ptr) + ci * 32),
-                           (F32C && p.out_fp32) ? 1 : 0);
-              }
-            }
-          }
-        }
-      }
-      // all TMEM reads of this accumulator stage are complete -> hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CL) mbar_arrive_cluster(mapa_rank0(&tmem_empty[acc]));   // the leader waits for both CTAs' drains
-        else mbar_arrive(&tmem_empty[acc]);
-      }
-      if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CL) cluster_sync_all();   // no CTA leaves (or frees TMEM) while its peer may still signal / write into it
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CL) tmem_dealloc2(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
+  // ===================================================== consumers: MMA + epilogue
+  setmaxnreg_inc<232>();
+  const int cwg = wg - 1;                 // rows [64 cwg, +64) of every tile
+  const int lane = tid & 31;
+  float acc[NACC];
+  int stage = 0;
+  uint32_t phase = 0;
+  if constexpr (RESB) {
+    if (unit_first < total_units) mbar_wait(b_full, 0);
+  }
+  // accumulator fragment: acc[4i + 2h + e] = tile row r_lo + 8h, column 8i + cq + e
+  const int r_lo = cwg * 64 + (tid >> 5) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const int esz = ((F & F_F32) != 0 && p.out_fp32) ? 4 : 2;
+  const bool ovec = !WS && ((reinterpret_cast<uintptr_t>(p.out) | static_cast<uintptr_t>(p.ldo * esz)) & (2 * esz - 1)) == 0;
+  const bool wvec = WS && !p.swap && ((reinterpret_cast<uintptr_t>(p.ws) | static_cast<uintptr_t>(p.ws_ld * 4)) & 7) == 0;
+
+  for (int unit = unit_first; unit < total_units; unit += unit_step) {
+    const TileCoord t = work_of(unit);
+    int k0, k1;
+    split_range(p, t.split, k0, k1);
+    if (k1 <= k0) {
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    }
+    int held = -1;   // ring slot whose MMAs may still be in flight
+    for (int kb = k0; kb < k1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cwg * (64 * 128);
+      const uint32_t sb = RESB ? smem_u32(sB_res + kb * B_BYTES) : smem_u32(smem + stage * STAGE_BYTES + A_BYTES);
+      const uint64_t da = gmma_desc_kmajor(sa), db = gmma_desc_kmajor(sb);
+      wgmma_fence_operand(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / WGMMA_K; ++k)
+        Wgmma<BLOCK_N>::ss(acc, da + 2 * k, db + 2 * k, (kb > k0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_fence_operand(acc);
+      wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot can be refilled
+      if (held >= 0 && lane == 0) mbar_arrive(&empty_bar[held]);
+      held = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operand(acc);
+    if (held >= 0 && lane == 0) mbar_arrive(&empty_bar[held]);
+
+    // ---------------- epilogue, straight from the accumulator registers
+    if (p.dbg & 1) continue;
+    const int col0 = t.n_blk * BLOCK_N;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int orow = tile_row_to_orow(p, t.m_blk, r_lo + 8 * h);
+      if (orow < 0) continue;
+      if constexpr (WS) {
+        float* wsp = p.ws + static_cast<size_t>(t.split) * p.ws_split_stride;
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 8; ++i) {
+          const int col = col0 + 8 * i + cq;
+          const float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          if (col >= p.N) continue;
+          const bool two = col + 1 < p.N;
+          if (p.swap) {
+            // C[token = col, feature = orow]
+            wsp[static_cast<size_t>(col) * p.ws_ld + orow] = v0;
+            if (two) wsp[static_cast<size_t>(col + 1) * p.ws_ld + orow] = v1;
+          } else {
+            float* dst = wsp + static_cast<size_t>(orow) * p.ws_ld + col;
+            if (two && wvec) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+            else { dst[0] = v0; if (two) dst[1] = v1; }
+          }
+        }
+      } else {
+        float rs = 1.f;
+        if constexpr ((F & F_RS) != 0) {
+          if (p.rowscale != nullptr) rs = __ldg(p.rowscale + orow);
+        }
+        const bf16* rb = nullptr;
+        if constexpr ((F & F_RB) != 0) {
+          if (p.rowbias != nullptr) rb = p.rowbias + static_cast<size_t>(orow / p.rowbias_rows) * p.N;
+        }
+        auto add_bias = [&](int col, float v) {
+          if (p.bias != nullptr) v += __bfloat162float(p.bias[col]);
+          if constexpr ((F & F_RB) != 0) {
+            if (rb != nullptr) v += __bfloat162float(rb[col]);
+          }
+          return v;
+        };
+        if constexpr (GLU) {
+          // packed GLU: accumulator columns come in blocks of 32 = [16 x "a" | 16 x "b"] (N % 32 == 0); the "a" and "b"
+          // values of an output sit in the same thread, 8 fragment columns apart
+#pragma unroll
+          for (int q = 0; q < BLOCK_N / 32; ++q) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              const int ia = 4 * (4 * q + j) + 2 * h, ib = ia + 8;
+              const int ca = col0 + 32 * q + 8 * j + cq;
+              if (ca >= p.N) continue;
+              const float a0 = add_bias(ca, acc[ia] * rs), a1 = add_bias(ca + 1, acc[ia + 1] * rs);
+              const float b0 = add_bias(ca + 16, acc[ib] * rs), b1 = add_bias(ca + 17, acc[ib + 1] * rs);
+              float o0, o1;
+              if (p.glu == VB_GLU_SWIGLU) { o0 = silu(a0) * b0; o1 = silu(a1) * b1; }
+              else { o0 = a0 * gelu_erf_fast(b0); o1 = a1 * gelu_erf_fast(b1); }
+              epi_store2<F>(p, orow, (col0 + 32 * q) / 2 + 8 * j + cq, true, ovec, o0, o1);
+            }
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 8; ++i) {
+            const int col = col0 + 8 * i + cq;
+            if (col >= p.N) continue;
+            const bool two = col + 1 < p.N;
+            float v0 = add_bias(col, acc[4 * i + 2 * h] * rs);
+            float v1 = two ? add_bias(col + 1, acc[4 * i + 2 * h + 1] * rs) : 0.f;
+            if constexpr ((F & F_ACT) != 0) {
+              v0 = apply_act(v0, p.act);
+              v1 = apply_act(v1, p.act);
+            }
+            epi_store2<F>(p, orow, col, two, ovec, v0, v1);
+          }
+        }
+      }
+    }
   }
 }
 
-// shared memory of a resident-B launch: B slab + A ring + barriers + epilogue bias copies; 0 = does not fit
-template <int BN, int STAGES>
-constexpr int resb_smem(int nkb) {
-  return nkb * BN * BLOCK_K * 2 + STAGES * BLOCK_M * BLOCK_K * 2 + 1024 + 256 + NUM_EPI_WARPS * BN * 4;
+// shared memory of a launch: [RESB: B slab] + ring + barriers (+ 1 KB for the manual 1024-byte alignment)
+template <int BN, int STAGES, bool RESB>
+constexpr int gemm_smem(int nkb) {
+  return (RESB ? nkb * BN * BLOCK_K * 2 : 0) + STAGES * (BLOCK_M * BLOCK_K * 2 + (RESB ? 0 : BN * BLOCK_K * 2)) + 1024 + 256;
 }
 
 template <int BN, int STAGES, int F>
 int launch_v2_resb(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  const int smem = resb_smem<BN, STAGES>(p.num_k_blocks);
+  const int smem = gemm_smem<BN, STAGES, true>(p.num_k_blocks);
   if (smem > SMEM_LIMIT || p.a_mode != 0 || p.splits != 1) return VB_ERR_UNSUPPORTED;
   static bool attr_set = false;
   auto kern = gemm_v2_kernel<BN, STAGES, F, true>;
@@ -603,65 +346,9 @@ int launch_v2_resb(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParam
   return VB_OK;
 }
 
-// CTA-pair launch: grid = 2 x clusters (<= SM count), cluster dimension 2, PDL attribute when enabled
-template <int BN, int STAGES, int F>
-int launch_v2_cl(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  constexpr int smem = STAGES * (BLOCK_M * BLOCK_K * 2 + (BN / 2) * BLOCK_K * 2) + 1024 + 256 + NUM_EPI_WARPS * BN * 4;
-  static_assert(smem <= SMEM_LIMIT, "smem budget");
-  if (p.splits != 1) return VB_ERR_UNSUPPORTED;
-  static bool attr_set = false;
-  static int max_clusters = 0;
-  auto kern = gemm_v2_kernel<BN, STAGES, F, false, true>;
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
-    // co-resident pairs (a GPC with an odd number of usable SMs leaves one without a partner)
-    cfg.gridDim = dim3(2 * (vb_num_sms() / 2));
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) { (void)cudaGetLastError(); n = vb_num_sms() / 2; }
-    max_clusters = n < vb_num_sms() / 2 ? n : vb_num_sms() / 2;
-    attr_set = true;
-  }
-  const int units = ((p.m_blocks + 1) >> 1) * p.n_blocks;
-  int clusters = max_clusters;
-  if (clusters > units) clusters = units;
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = vb_pdl_enabled() ? 2 : 1;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, kern, ta, tb, p);
-  if (le != cudaSuccess) { vb_set_last_error(le); return VB_ERR_CUDA; }
-  return VB_OK;
-}
-
-template <int BN, int STAGES>
-int dispatch_v2_cl(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  if (need == 0) return launch_v2_cl<BN, STAGES, 0>(ta, tb, p, stream);
-  if (need == F_RES) return launch_v2_cl<BN, STAGES, F_RES>(ta, tb, p, stream);
-  if (need == F_GLU) return launch_v2_cl<BN, STAGES, F_GLU>(ta, tb, p, stream);
-  if (need == F_ACT) return launch_v2_cl<BN, STAGES, F_ACT>(ta, tb, p, stream);
-  if (need == F_RB) return launch_v2_cl<BN, STAGES, F_RB>(ta, tb, p, stream);
-  if (need == (F_RB | F_RES)) return launch_v2_cl<BN, STAGES, F_RB | F_RES>(ta, tb, p, stream);
-  return VB_ERR_UNSUPPORTED;
-}
-
 template <int BN, int STAGES, int F>
 int launch_v2(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  constexpr int smem = STAGES * (BLOCK_M * BLOCK_K * 2 + BN * BLOCK_K * 2) + 1024 + 256 + NUM_EPI_WARPS * BN * 4;
+  constexpr int smem = gemm_smem<BN, STAGES, false>(0);
   static_assert(smem <= SMEM_LIMIT, "smem budget");
   static bool attr_set = false;
   auto kern = gemm_v2_kernel<BN, STAGES, F>;
@@ -687,27 +374,29 @@ int dispatch_v2_resb(int need, const CUtensorMap& ta, const CUtensorMap& tb, con
   return VB_ERR_UNSUPPORTED;
 }
 
-// variant of tile width BN covering the feature set `need` (F_* mask; F_WS selects the split-K variant)
+// variant of tile width BN covering the feature set `need` (F_* mask; F_WS selects the partials variant); `generic`
+// takes the variants that resolve every feature at run time
 template <int BN, int STAGES>
-int dispatch_v2(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+int dispatch_v2(int need, bool generic, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
   if (need & F_WS) return launch_v2<BN, STAGES, F_WS>(ta, tb, p, stream);
-  if (need == 0) return launch_v2<BN, STAGES, 0>(ta, tb, p, stream);
-  if (need == F_ACT) return launch_v2<BN, STAGES, F_ACT>(ta, tb, p, stream);
-  if (need == F_RES) return launch_v2<BN, STAGES, F_RES>(ta, tb, p, stream);
-  if (need == F_GLU) return launch_v2<BN, STAGES, F_GLU>(ta, tb, p, stream);
-  if (need == (F_GLU | F_RS)) return launch_v2<BN, STAGES, F_GLU | F_RS>(ta, tb, p, stream);
-  if (need == F_RS) return launch_v2<BN, STAGES, F_RS>(ta, tb, p, stream);
-  if (need == F_RB) return launch_v2<BN, STAGES, F_RB>(ta, tb, p, stream);
+  if (!generic) {
+    if (need == 0) return launch_v2<BN, STAGES, 0>(ta, tb, p, stream);
+    if (need == F_ACT) return launch_v2<BN, STAGES, F_ACT>(ta, tb, p, stream);
+    if (need == F_RES) return launch_v2<BN, STAGES, F_RES>(ta, tb, p, stream);
+    if (need == F_GLU) return launch_v2<BN, STAGES, F_GLU>(ta, tb, p, stream);
+    if (need == (F_GLU | F_RS)) return launch_v2<BN, STAGES, F_GLU | F_RS>(ta, tb, p, stream);
+    if (need == F_RS) return launch_v2<BN, STAGES, F_RS>(ta, tb, p, stream);
+    if (need == F_RB) return launch_v2<BN, STAGES, F_RB>(ta, tb, p, stream);
+  }
   if (need & F_GLU) return launch_v2<BN, STAGES, F_ALL_GLU>(ta, tb, p, stream);
   return launch_v2<BN, STAGES, F_ALL>(ta, tb, p, stream);
 }
 
-int launch_gemm_v2_cl(int bn, int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
 int launch_gemm_v2_resb(int bn, int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
-int launch_gemm_v2_256(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
-int launch_gemm_v2_160(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
-int launch_gemm_v2_128(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
-int launch_gemm_v2_64(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
-int launch_gemm_v2_32(int need, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
+int launch_gemm_v2_256(int need, bool generic, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
+int launch_gemm_v2_160(int need, bool generic, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
+int launch_gemm_v2_128(int need, bool generic, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
+int launch_gemm_v2_64(int need, bool generic, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
+int launch_gemm_v2_32(int need, bool generic, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream);
 
 }  // namespace vb

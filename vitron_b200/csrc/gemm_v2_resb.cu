@@ -1,4 +1,4 @@
-// vitron_b200 — gemm_v2 "resident B" instantiations (small-K GEMMs: the weight n-block stays in shared memory); see gemm_v2.cuh.
+// vitron_b200 — wgmma GEMM "resident B" instantiations (small-K GEMMs: the weight n-block stays in shared memory); see gemm_v2.cuh.
 #include "gemm_v2.cuh"
 
 namespace vb {
@@ -13,9 +13,9 @@ int launch_gemm_v2_resb(int bn, int need, const CUtensorMap& ta, const CUtensorM
 }
 int resb_smem_bytes(int bn, int nkb) {
   switch (bn) {
-    case 256: return resb_smem<256, 3>(nkb);
-    case 160: return resb_smem<160, 6>(nkb);
-    case 128: return resb_smem<128, 3>(nkb);
+    case 256: return gemm_smem<256, 3, true>(nkb);
+    case 160: return gemm_smem<160, 6, true>(nkb);
+    case 128: return gemm_smem<128, 3, true>(nkb);
     default: return 1 << 30;
   }
 }

@@ -3,14 +3,14 @@
 //   out[M, N'] = epilogue( X[M, K] · W[N, K]^T ),  M <= 16
 //
 // At M = 8 every weight byte is used for 8 FMAs: the op is HBM-bound (13 GB of Vicuna-7B weights per
-// decoded token), so the design goal is bytes in flight, not tensor throughput: no TMEM/TMA
+// decoded token), so the design goal is bytes in flight, not tensor throughput: no TMA
 // prologue, no split-K workspace, one launch with the epilogue fused. Each CTA owns 16 (or 32, for
 // the packed-GLU layout) consecutive output features and the whole K range; its 8 warps split K,
 // stream their weight rows straight from global memory with 16-byte loads (2 x 64-byte segments
 // per row per step, 8 loads in flight per thread), multiply on the legacy m16n8k16 tensor path
 // (weights = A, tokens = B; the k order inside a 64-chunk is permuted identically on both
 // operands so that each thread's fragment is contiguous in memory), and reduce across warps in smem.
-// Replaces the same nn.Linear call sites as gemm_tcgen05.cu for tiny M.
+// Replaces the same nn.Linear call sites as gemm.cu for tiny M.
 #include "common.cuh"
 #include "vitron_b200.h"
 #include <type_traits>
@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(256, 2) gemv_bf16_kernel(const GemvParams p) {
 
 using namespace vb;
 
-// internal entry used by vb200_gemm_bf16 (gemm_tcgen05.cu) for M <= 16
+// internal entry used by vb200_gemm_bf16 (gemm.cu) for M <= 16
 int vb_launch_gemv(const void* A, int64_t lda, const void* W, int64_t ldw, void* out, int64_t ldo, int64_t M,
                    int64_t N, int64_t K, const vb_epilogue* e, cudaStream_t stream) {
   GemvParams p;

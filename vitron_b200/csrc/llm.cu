@@ -114,7 +114,7 @@ __global__ void rope_table_kernel(const int32_t* __restrict__ positions, float* 
 }
 
 template <bool ROPE, int MAX_TRIPS>
-__global__ void __launch_bounds__(DEC_THREADS, 4)   // 4 CTAs per SM: the one-wave split policy counts on 4 x 148 slots
+__global__ void __launch_bounds__(DEC_THREADS, 4)   // 4 CTAs per SM: the one-wave split policy counts on 4 x (SM count) slots
 attn_decode_kernel(const bf16* __restrict__ q, long long ld_q, bf16* __restrict__ k_pages,
                    bf16* __restrict__ v_pages, const int32_t* __restrict__ block_table, int max_pages,
                    const int32_t* __restrict__ kv_len, int H, int page_size, float scale, int splits, int per,
@@ -135,7 +135,6 @@ attn_decode_kernel(const bf16* __restrict__ q, long long ld_q, bf16* __restrict_
     const int pi = c0 / 64 + i;
     pg[i] = (pi < max_pages && i * 64 < per) ? bt[pi] : 0;
   }
-  pdl_trigger();
   // L2 prefetch of this CTA's first page (K and V, 16 KB each for this head) while the predecessor (the qkv projection,
   // which does not touch the cache) drains: pages of earlier tokens are constant during the step. One 128-byte line per
   // 4 lanes; the remaining trips are prefetched two trips ahead inside the loop.
@@ -149,6 +148,11 @@ attn_decode_kernel(const bf16* __restrict__ q, long long ld_q, bf16* __restrict_
   if (per > 0) prefetch_page(pg[0]);
   if (MAX_TRIPS > 1 && per > 64) prefetch_page(pg[1]);
   pdl_wait();
+  // Dependents are released only now, after this grid's own dependency wait: released at kernel entry, the o-projection
+  // GEMM and its split-K reduce (which rewrite the shared GEMM workspace and the hidden state) were let in while the qkv
+  // projection that feeds this kernel was still in flight, and decode steps at batch >= 17 (GEMM, not GEMV, path) gave
+  // different tokens from run to run.
+  pdl_trigger();
   const int len = kv_len[b];
   const int c1 = min(len, c0 + per);
 
@@ -469,9 +473,8 @@ extern "C" int vb200_rope_kv_append(void* qkv, int64_t ld_qkv, const int32_t* po
 static int decode_splits(int64_t max_kv_len, int64_t bh) {
   // As few splits as still give every SM its 4 resident CTAs (113 registers x 128 threads): the whole grid runs as ONE
   // wave and the per-CTA fixed cost (q load + RoPE, partial write, arrival atomics, merge) is paid once per 512 keys, with
-  // the next page already on its way to L2 while a 64-key trip is processed. Measured at B = 8, 896-token cache inside
-  // the real decode step (profiles/r02_decode_attention_split_keys.txt): 128 / 256 / 512 keys per split -> 3.77 / 3.68 /
-  // 3.58 ms per token. Small batches get more, shorter splits (down to 128 keys) to fill the machine.
+  // the next page already on its way to L2 while a 64-key trip is processed. Small batches get more, shorter splits (down
+  // to 128 keys) to fill the machine.
   static int keys_env = -1;   // VB200_DEC_SPLIT_KEYS = 128 / 256 / 512 pins the split length (tuning aid)
   if (keys_env < 0) {
     const char* e = getenv("VB200_DEC_SPLIT_KEYS");

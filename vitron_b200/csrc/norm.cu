@@ -326,12 +326,13 @@ __device__ __forceinline__ void gn_accumulate(const uint4 u, float (&s)[8], floa
   f = unpack_bf16(u.w); s[6] += f.x; q[6] += f.x * f.x; s[7] += f.y; q[7] += f.y * f.y;
 }
 
-constexpr int GN_REPL = 8;  // replicated group accumulators: 148 CTAs adding into ONE address per group serialise in L2
-
+// The CTAs of a sample publish their group partial sums in slots of their own (no atomics) and every CTA adds the slots
+// of its sample in one fixed order, so the statistics — and everything downstream of them — are bit-identical from run
+// to run.
 struct GnWs {
-  float* sums;      // [n][GN_REPL][groups][2]
+  float* sums;      // [n * ctas per sample][groups][2]: one slot per CTA, overwritten by every launch
   int* arrived;     // [n]  CTAs of the sample that published their sums
-  int* readers;     // [n]  CTAs of the sample that consumed the sums (the last one cleans up)
+  int* readers;     // [n]  CTAs of the sample that consumed the sums (the last one resets both counters)
 };
 
 // SiLU with ONE MUFU op per element: x * sigmoid(x) = 0.5 x (1 + tanh(x / 2)); tanh.approx.f32 has ~2^-11 relative error,
@@ -433,9 +434,9 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
   __syncthreads();
   const int cpg = c / groups;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;  // blockDim is a multiple of 32
-  float* gs = ws.sums + static_cast<size_t>(n) * GN_REPL * groups * 2;          // all replicas of this sample
-  float* gs_mine = gs + static_cast<size_t>(blockIdx.x % GN_REPL) * groups * 2;  // the replica this CTA adds into
   const int ctas = gridDim.x;
+  const float* gs = ws.sums + static_cast<size_t>(n) * ctas * groups * 2;           // the slots of this sample
+  float* gs_mine = ws.sums + (static_cast<size_t>(n) * ctas + blockIdx.x) * groups * 2;  // this CTA's slot
   for (int g = warp; g < groups; g += nwarps) {
     float as = 0.f, aq = 0.f;
     const int items = rpp * cpg;
@@ -449,8 +450,8 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
     aq = warp_sum(aq);
     if (lane == 0) {
       if (ctas > 1) {
-        atomicAdd(gs_mine + g * 2, as);
-        atomicAdd(gs_mine + g * 2 + 1, aq);
+        gs_mine[g * 2] = as;
+        gs_mine[g * 2 + 1] = aq;
       } else {  // the whole sample is this CTA: no global round trip
         gsum[g * 2] = as;
         gsum[g * 2 + 1] = aq;
@@ -467,14 +468,15 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
     }
   }
   __syncthreads();
-  // ---- group sums of the sample = sum of the replicas -> gsum; then the per-channel affine into smem (`part` is free:
-  // every warp passed the barrier above after its reads)
+  // ---- group sums of the sample = sum of its CTAs' slots -> gsum, in a fixed order (lane l adds slots l, l + 32, ...,
+  // then a fixed shuffle tree); then the per-channel affine into smem (`part` is free: every warp passed the barrier
+  // above after its reads)
   if (ctas > 1) {
-    for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) {
+    for (int i = warp; i < groups * 2; i += nwarps) {
       float a = 0.f;
-#pragma unroll
-      for (int rp = 0; rp < GN_REPL; ++rp) a += __ldcg(gs + static_cast<size_t>(rp) * groups * 2 + i);
-      gsum[i] = a;
+      for (int k = lane; k < ctas; k += 32) a += __ldcg(gs + static_cast<size_t>(k) * groups * 2 + i);
+      a = warp_sum(a);
+      if (lane == 0) gsum[i] = a;
     }
     __syncthreads();
   }
@@ -518,13 +520,10 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
   }
   if (ctas > 1 && threadIdx.x == 0) {
     // every thread of this CTA read the sums before the affine barrier: the last CTA of the sample to get here hands the
-    // workspace back zeroed (done after this thread's share of the apply pass so that it delays nothing)
+    // counters back zeroed (done after this thread's share of the apply pass so that it delays nothing)
     __threadfence();
     const int prev = atomicAdd(ws.readers + n, 1);
     if (prev == ctas - 1) {
-      float4* z = reinterpret_cast<float4*>(gs);
-      for (int i = 0; i < GN_REPL * groups * 2 / 4; ++i) z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int i = (GN_REPL * groups * 2 / 4) * 4; i < GN_REPL * groups * 2; ++i) gs[i] = 0.f;
       ws.arrived[n] = 0;
       ws.readers[n] = 0;
     }
@@ -562,10 +561,18 @@ constexpr int GN_DYN_SMEM_MAX = 220 * 1024;  // dynamic smem budget of gn_onepas
 
 static size_t gn_align16(size_t v) { return (v + 15) & ~static_cast<size_t>(15); }
 
+// The counters live in a FIXED-size prefix, the per-CTA sum slots behind it: one workspace serves calls of any n / groups
+// without a call's counters ever landing on another call's (stale) sums. Larger batches run in chunks of GN_MAX_N samples.
+constexpr int64_t GN_MAX_N = 1024;
+constexpr size_t GN_COUNTER_BYTES = 2 * GN_MAX_N * sizeof(int);   // arrived[GN_MAX_N] | readers[GN_MAX_N]
+
 extern "C" size_t vb200_groupnorm_workspace_size(int64_t n, int64_t groups, int64_t c) {
-  // [group sums | arrival counters | reader counters]; zero-fill ONCE before first use, the kernel leaves it zeroed
+  // [arrival counters | reader counters | per-CTA group sums]; zero-fill ONCE before first use, the kernel leaves the
+  // counters zeroed and overwrites the sum slots it reads (a launch has at most max(n, SM count) CTAs: gn_plan)
   (void)c;
-  return gn_align16(static_cast<size_t>(n) * GN_REPL * groups * 2 * sizeof(float)) + 2 * gn_align16(static_cast<size_t>(n) * sizeof(int));
+  if (n > GN_MAX_N) n = GN_MAX_N;
+  const int64_t ctas = n > vb_num_sms() ? n : vb_num_sms();
+  return GN_COUNTER_BYTES + gn_align16(static_cast<size_t>(ctas) * groups * 2 * sizeof(float));
 }
 
 template <int ACT, bool CACHED>
@@ -637,14 +644,24 @@ extern "C" int vb200_groupnorm_nhwc(const void* x, const void* weight, const voi
   VB_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0);
   const size_t need = vb200_groupnorm_workspace_size(n, groups, c);
   if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15) != 0) return VB_ERR_WORKSPACE;
+  if (n > GN_MAX_N) {
+    for (int64_t s0 = 0; s0 < n; s0 += GN_MAX_N) {
+      const int64_t ns = n - s0 < GN_MAX_N ? n - s0 : GN_MAX_N;
+      const size_t off = static_cast<size_t>(s0) * spatial * c;
+      const int r = vb200_groupnorm_nhwc(reinterpret_cast<const bf16*>(x) + off, weight, bias, reinterpret_cast<bf16*>(out) + off, ns,
+                                         spatial, c, groups, eps, act, workspace, workspace_bytes, stream);
+      if (r != VB_OK) return r;
+    }
+    return VB_OK;
+  }
   GnWs ws;
   char* wsp = reinterpret_cast<char*>(workspace);
-  ws.sums = reinterpret_cast<float*>(wsp);
-  ws.arrived = reinterpret_cast<int*>(wsp + gn_align16(static_cast<size_t>(n) * GN_REPL * groups * 2 * sizeof(float)));
-  ws.readers = reinterpret_cast<int*>(reinterpret_cast<char*>(ws.arrived) + gn_align16(static_cast<size_t>(n) * sizeof(int)));
+  ws.arrived = reinterpret_cast<int*>(wsp);
+  ws.readers = ws.arrived + GN_MAX_N;
+  ws.sums = reinterpret_cast<float*>(wsp + GN_COUNTER_BYTES);
   GnPlan pl = gn_plan(n, spatial, c);
   if (!pl.cached && n > 1) {
-    // The slabs of all n samples do not fit the GPU's shared memory at once (batch-2 UNet levels: 52 MB against 148 x 220 KB):
+    // The slabs of all n samples do not fit the GPU's shared memory at once (batch-2 UNet levels: 52 MB against 132 x 220 KB):
     // rather than reading x twice, normalise the samples in chunks whose slabs DO fit, one launch per chunk (measured at
     // [2, 40960, 320]: 48 us in one two-pass launch, 2 x 18 us cached). Every chunk uses the same self-zeroing workspace.
     int64_t nc = n;

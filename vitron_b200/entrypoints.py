@@ -1,5 +1,5 @@
 """The module-level entry points of the reference's `modules/*` with their own signatures (SURVEY.md §8b face 1), as thin
-orchestration over the B200 pipelines of this package:
+orchestration over the CUDA pipelines of this package:
 
   reference                                                                 here
   ------------------------------------------------------------------------  --------------------------------------------
@@ -94,7 +94,7 @@ def draw_masks_from_boxes(boxes, size):
 
 
 def load_ckpt(config, state_dict, device="cuda"):
-    """task_grounded_generation.py:66-81 on the B200 modules: `config` provides `model` (UNetModel kwargs), `autoencoder`
+    """task_grounded_generation.py:66-81 on the CUDA modules: `config` provides `model` (UNetModel kwargs), `autoencoder`
     (ddconfig, embed_dim, scale_factor), `alpha_scale`; `state_dict` the four sub-dicts. The text encoder (CLIP text
     transformer) is third-party and injected as `config['text_encoder']` (object with `.encode(list[str])`)."""
     from .autoencoder import AutoencoderKL

@@ -4,9 +4,9 @@ Drop-in for modules/SEEM/demo_code/xdecoder/backbone/focal.py: `FocalNet` (:340-
 constructor keywords, state-dict names and `forward(x) -> {"res2".."res5": [B, C_i, H_i, W_i]}`; `D2FocalNet`
 (:598-672) builds it from the `cfg['BACKBONE']['FOCAL']` block of configs/seem/seem_focall_lang.yaml:29-47.
 
-B200 design (NHWC bf16 end to end, no NCHW round trips — the reference permutes to NCHW and back inside every
+Design (NHWC bf16 end to end, no NCHW round trips — the reference permutes to NCHW and back inside every
 FocalModulation, :101,114):
-  * every Linear / 1x1 conv is the tcgen05 GEMM (`f` is padded to N = 2C+8 so q | ctx | gates are column
+  * every Linear / 1x1 conv is the wgmma GEMM (`f` is padded to N = 2C+8 so q | ctx | gates are column
     slices of ONE output buffer: no torch.split copy); fc1 carries the exact-erf GELU in its epilogue;
   * the focal levels are a register-sliding-window depthwise conv kernel with the GELU fused (FFMA2),
     reading its first input in place from the `f` output (strided view);

@@ -62,7 +62,7 @@ def alpha_generator(length, type=(1, 0, 0)):
 
 
 def set_alpha_scale(model, alpha_scale):
-    """evaluator.py:35-39 on the B200 UNetModel: `scale` of every GatedSelfAttentionDense fuser."""
+    """evaluator.py:35-39 on the CUDA UNetModel: `scale` of every GatedSelfAttentionDense fuser."""
     w = getattr(model, "w", None)
     if w is None:
         raise RuntimeError("set_alpha_scale: load_state_dict() first")

@@ -7,8 +7,8 @@ FourierEmbedder (diffusionmodules/util.py:160-180, 12-26): same constructor keyw
 `forward(input)` with the reference's input dict (`x`, `timesteps`, `context`, `boxes`, `masks`, `text_embeddings`,
 optional `inpainting_extra_input`). The transformer blocks are `vitron_b200.gligen.BasicTransformerBlock` (row a12).
 
-B200 design: NHWC bf16 end to end (the reference flips 'b c h w' <-> 'b (h w) c' around every SpatialTransformer);
-3x3 convs, stride-2 downsample and the conv after the nearest upsample are the TMA implicit-GEMM tcgen05 kernel; the
+Design: NHWC bf16 end to end (the reference flips 'b c h w' <-> 'b (h w) c' around every SpatialTransformer);
+3x3 convs, stride-2 downsample and the conv after the nearest upsample are the TMA implicit-GEMM wgmma kernel; the
 time-embedding projections of ALL ResBlocks are one GEMM per forward and enter conv1 as a per-sample row bias in its
 epilogue; GroupNorm(32)+SiLU is one fused kernel; skip 1x1 convs, proj_in / proj_out are GEMMs on the pixel rows with
 the residual in the epilogue.

@@ -61,7 +61,7 @@ def reserve_decode_workspace(max_batch, n_heads, head_dim, device):
 class pdl:
     """Context manager: launch the vitron_b200 kernels issued inside with programmatic dependent launch (every kernel
     launched through vb_launch starts with griddepcontrol.launch_dependents / .wait): consecutive kernels of a stream or of
-    a captured CUDA graph overlap launch latency and prologue (barrier init, TMEM allocation) with the predecessor's tail."""
+    a captured CUDA graph overlap launch latency and prologue (barrier init, tensor-map prefetch) with the predecessor's tail."""
 
     def __init__(self, enabled=True):
         self.enabled, self.prev = enabled, None
@@ -138,7 +138,7 @@ def pack_glu_weight(w_a, w_b):
 
 def gemm(a, w, bias=None, act=ACT_NONE, glu=GLU_NONE, residual=None, alpha=1.0, rowbias=None,
          rowbias_rows=0, out=None, out_fp32=False, rowscale=None, rms_eps=0.0):
-    """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T) on tcgen05 tensor cores."""
+    """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T) on wgmma tensor cores."""
     lib = _lib.load()
     a2, lda = _rows2d(a)
     _req(a2.dtype == BF16 and w.dtype == BF16, "gemm operands must be bf16")
@@ -332,12 +332,12 @@ def attention(q, k, v, scale=None, causal=False, kv_len=None, mask=None, out=Non
 
 
 def set_attention_impl(impl):
-    """0 = automatic, 1 = mma.sync kernel only, 2 = tcgen05 kernel whenever the shape is supported."""
+    """0 = automatic, 1 = mma.sync kernel only, 2 = wgmma kernel whenever the shape is supported."""
     check(_lib.load().vb200_set_attention_impl(int(impl)), "vb200_set_attention_impl")
 
 
 def attention_watchdog():
-    """(site, block, thread) of the first expired wait in the tcgen05 attention kernel since the last call;
+    """(site, block, thread) of the first expired wait in the wgmma attention kernel since the last call;
     site 0 = none. Synchronises."""
     import ctypes
     buf = (ctypes.c_uint32 * 3)()

@@ -14,7 +14,7 @@ Drop-ins for modules/SEEM/demo_code/xdecoder:
 State-dict names are the reference's. Interactive prompts (spatial / grounding / visual / audio
 `extra` keys) are not on the BASELINE path and raise NotImplementedError (DESIGN.md "next").
 
-B200 design: NHWC bf16 throughout; the K/V projections of the memory for the 3 layers that share a
+Design: NHWC bf16 throughout; the K/V projections of the memory for the 3 layers that share a
 feature level are ONE grouped GEMM per level (N = 3 x 512); the mask head `einsum('bqc,bchw->bqhw')`
 is a GEMM against the NHWC mask_features viewed as [HW, C]; the next layer's bool attention mask
 (bilinear resize, sigmoid < 0.5, fully-masked-row reset) is one fused kernel with the threshold

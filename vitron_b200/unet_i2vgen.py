@@ -7,10 +7,10 @@ tools/modules/unet/util.py: ResBlock :610-730, TemporalConvBlock_v2 :1347-1392, 
 :311-373, BasicTransformerBlock :510-540, GEGLU/FeedForward :543-577, TemporalTransformer :992-1089,
 Upsample/Downsample :579-607,732-756, TransformerV2 :1129-1148, sinusoidal_embedding :177-189.
 
-B200 design: activations stay NHWC bf16 `[(b f), h, w, c]` end to end — the reference's ~40
+Design: activations stay NHWC bf16 `[(b f), h, w, c]` end to end — the reference's ~40
 `rearrange(...).contiguous()` layout flips per forward disappear because (i) Conv2d 3x3 / Conv3d
 (3,1,1) are im2col-free implicit GEMMs reading the NHWC tensor through 4-D TMA maps, (ii) every
-Linear is a row-wise tcgen05 GEMM with bias / GEGLU / residual fused, (iii) temporal attention reads
+Linear is a row-wise wgmma GEMM with bias / GEGLU / residual fused, (iii) temporal attention reads
 its length-f sequences with strides. All 22 ResBlock time-embedding projections are one GEMM.
 The tiny x-independent local-image adapter (4..32 channels, <0.01 % of FLOPs) runs once per
 conditioning through torch ops and is cached.

@@ -7,7 +7,7 @@ Drop-in for the reference's `LanguageBindImageTower` / `LanguageBindVideoTower`
 MLP, modeling_video.py:83-134).  Same forward signatures and attributes; parameters are read from
 a state dict with the reference's names (SURVEY.md Appendix B).
 
-Mechanism differences: patch-embed is patchify + tcgen05 GEMM, q/k/v is one fused GEMM, attention
+Mechanism differences: patch-embed is patchify + wgmma GEMM, q/k/v is one fused GEMM, attention
 never materialises S x S scores, bias/activation/residual live in GEMM epilogues, only the layers
 that influence `hidden_states[select_layer]` are executed (the reference computes and discards the
 rest), and the video tower's two `rearrange` transposes per layer are replaced by strided attention.

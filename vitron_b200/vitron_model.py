@@ -1,4 +1,4 @@
-"""VitronLlamaForCausalLM — drop-in for the reference's LlavaLlamaForCausalLM on B200 kernels.
+"""VitronLlamaForCausalLM — drop-in for the reference's LlavaLlamaForCausalLM on H100 kernels.
 
 Mirrors vitron/model/language_model/llava_llama.py:40-114 (`forward`, `generate` via HF
 GenerationMixin, `prepare_inputs_for_generation`) and vitron/model/llava_arch.py:153-573
