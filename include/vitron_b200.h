@@ -216,6 +216,31 @@ int vb200_argmax_advance(const float* logits, int64_t ld, int64_t rows, int64_t 
                          int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
                          int64_t log_stride, const int32_t* prompt_len, cudaStream_t stream);
 
+/* Sampling parameters, read by the kernel from DEVICE memory (one captured decode graph serves every setting). */
+typedef struct vb_sample_params {
+  float temperature; /* > 0; callers clamp with max(T, 1e-6) */
+  int32_t top_k;     /* 0 = off; k >= number of non-NaN logits is off too */
+  float top_p;       /* >= 1 = off */
+  uint32_t reserved;
+  uint64_t seed;     /* Philox key: (low 32 bits, high 32 bits) */
+} vb_sample_params;
+
+/* sampled step: the same bookkeeping as vb200_argmax_advance (out_idx optional) with the token drawn per row b from
+ *   1. z_i = logit_i / T; NaN logits are never drawn; a row with no number gives token 0;
+ *   2. top-k: keep i iff z_i >= the k-th largest z (ties at the threshold are kept);
+ *   3. p_i = exp(z_i - max z) over the kept set;
+ *   4. top-p: keep i iff (kept mass of p_j > p_i) / (kept total) < top_p (value-based: ties stay together, the
+ *      maximum always stays; HF TopPLogitsWarper with min_tokens_to_keep = 1);
+ *   5. x = Philox4x32-10(counter (t, b, 0, 0), key (seed_lo, seed_hi)), t = kv_len[b] - prompt_len[b] (0 without
+ *      kv_len / prompt_len: the token of the prefill logits); u = (x[0] >> 8) * 2^-24; the token is the first kept
+ *      index, in vocabulary order, whose inclusive prefix sum of kept p exceeds u * (sum of kept p).
+ * Masses are fixed point (2^-40 units): the result does not depend on the order of the device's sums. One CTA per
+ * row, the row staged in shared memory: n <= 49152 (else VB_ERR_UNSUPPORTED). Stands in for HF
+ * GenerationMixin.sample's logits warpers + torch.multinomial and its per-token host round trip. */
+int vb200_sample_advance(const float* logits, int64_t ld, int64_t rows, int64_t n, const vb_sample_params* params,
+                         int64_t* out_idx, int32_t* next_src, int32_t* positions, int32_t* kv_len,
+                         int64_t* token_log, int64_t log_stride, const int32_t* prompt_len, cudaStream_t stream);
+
 /* ---- vision / diffusion glue (vision.cu) ----------------------------------------------------
  * patchify: NCHW pixels -> [nb*gh*gw, kpad] rows ordered (c, py, px) for the patch-embed GEMM
  * (HF CLIPVisionEmbeddings Conv2d(3,1024,14,14,bias=False)); vit_embed adds cls + position and

@@ -434,6 +434,248 @@ argmax_advance_kernel(const float* __restrict__ logits, long long ld, int n, int
   }
 }
 
+// ------------------------------------------------------------------ sampling (temperature, top-k, top-p, Philox draw)
+// One CTA per row; the row is staged in shared memory. Both cuts are radix selects over a 32-bit order key of the logit
+// (11 + 11 + 10 bit digits): top-k by per-bin counts, top-p by per-bin mass. Masses are fixed point (p * 2^40, p <= 1) so
+// every sum is an integer sum: the same logits give the same token on every run, whatever the order of the atomics.
+constexpr int SMP_THREADS = 1024;
+constexpr int SMP_BINS = 2048;
+constexpr int SMP_MAX_N = 49152;               // 192 KB of staged row + 24 KB of histograms fit the 227 KB of an SM
+constexpr float SMP_FIX = 1099511627776.0f;    // 2^40
+
+// monotone map float -> uint32 (larger value, larger key); NaN -> 0, below every number (-inf -> 0x007fffff); -0 == +0
+__device__ __forceinline__ uint32_t order_key(float v) {
+  if (v != v) return 0u;
+  const uint32_t u = v == 0.f ? 0u : __float_as_uint(v);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// Random123 philox4x32-10
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+template <typename T>
+__device__ __forceinline__ T warp_inclusive_scan(T v) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T x = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += x;
+  }
+  return v;
+}
+
+// exclusive prefix of v over threadIdx order (blockDim == 1024); *total gets the block sum. buf: 33 entries.
+template <typename T>
+__device__ T block_exclusive_scan(T v, T* buf, T* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T inc = warp_inclusive_scan(v);
+  if (lane == 31) buf[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    const T w = buf[lane];
+    const T wi = warp_inclusive_scan(w);
+    buf[lane] = wi - w;
+    if (lane == 31) buf[32] = wi;
+  }
+  __syncthreads();
+  const T r = buf[warp] + inc - v;
+  *total = buf[32];
+  __syncthreads();
+  return r;
+}
+
+__global__ void __launch_bounds__(SMP_THREADS, 1)
+sample_advance_kernel(const float* __restrict__ logits, long long ld, int n, const vb_sample_params* __restrict__ prm,
+                      int64_t* __restrict__ out_idx, int32_t* __restrict__ next_src, int32_t* __restrict__ positions,
+                      int32_t* __restrict__ kv_len, int64_t* __restrict__ token_log, int log_stride,
+                      const int32_t* __restrict__ prompt_len) {
+  extern __shared__ float srow[];
+  __shared__ uint32_t h_cnt[SMP_BINS];
+  __shared__ unsigned long long h_mass[SMP_BINS];
+  __shared__ unsigned long long s_u64[33];
+  __shared__ uint32_t s_u32[33];
+  __shared__ float s_f32[32];
+  __shared__ uint32_t s_bin;
+  __shared__ unsigned long long s_above;
+  __shared__ int s_tok;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  pdl_wait();      // the logits and the decode state come from the predecessors
+  pdl_trigger();
+  const float* row = logits + b * ld;
+
+  // ---- stage the row (rows of an odd-V matrix are only 4-byte aligned: scalar head, float4 body, scalar tail)
+  float mx = -INFINITY;
+  uint32_t valid = 0;
+  auto take = [&](int i, float v) {
+    srow[i] = v;
+    if (v == v) { mx = fmaxf(mx, v); ++valid; }
+  };
+  int head = static_cast<int>(((16u - (reinterpret_cast<uintptr_t>(row) & 15u)) & 15u) >> 2);
+  if (head > n) head = n;
+  const int nvec = (n - head) >> 2;
+  if (tid < head) take(tid, row[tid]);
+  const float4* row4 = reinterpret_cast<const float4*>(row + head);
+  for (int j = tid; j < nvec; j += SMP_THREADS) {
+    const float4 v = row4[j];
+    const int i = head + 4 * j;
+    take(i, v.x); take(i + 1, v.y); take(i + 2, v.z); take(i + 3, v.w);
+  }
+  for (int i = head + 4 * nvec + tid; i < n; i += SMP_THREADS) take(i, row[i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    valid += __shfl_xor_sync(0xffffffffu, valid, o);
+  }
+  if (lane == 0) { s_f32[warp] = mx; s_u32[warp] = valid; }
+  __syncthreads();
+  mx = s_f32[lane];
+  valid = s_u32[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    valid += __shfl_xor_sync(0xffffffffu, valid, o);
+  }
+  __syncthreads();
+
+  int tok = 0;   // a row without a number samples token 0, like the arg-max
+  if (valid > 0) {
+    const float temp = prm->temperature, top_p = prm->top_p;
+    const int top_k = prm->top_k;
+    // p_i = exp(z_i - max z), z = logit / T, as fixed point; the maximum itself is exactly 1 (also for +-inf)
+    auto mass_of = [&](float v) -> unsigned long long {
+      const float p = v == mx ? 1.f : expf((v - mx) / temp);
+      return __float2ull_rn(p * SMP_FIX);
+    };
+    uint32_t thr = 1u;   // kept set = {i : order_key(logit_i) >= thr}; thr = 1 drops only the NaNs
+
+    // One radix level over the kept keys whose bits above `shift + width` equal `prefix`: histogram of the digit, then
+    // the lowest non-empty bin whose "before" value (count / mass of the kept keys in strictly higher bins, plus `above`)
+    // is still below `limit`. Returns that bin; s_above gets its "before" value.
+    auto radix_level = [&](uint32_t prefix, uint32_t himask, int shift, uint32_t dmask, bool by_mass,
+                           unsigned long long above, unsigned long long limit) -> uint32_t {
+      for (int i = tid; i < SMP_BINS; i += SMP_THREADS) { h_cnt[i] = 0; h_mass[i] = 0; }
+      if (tid == 0) s_bin = SMP_BINS;
+      __syncthreads();
+      for (int i = tid; i < n; i += SMP_THREADS) {
+        const float v = srow[i];
+        const uint32_t key = order_key(v);
+        if (key >= thr && (key & himask) == prefix) {
+          const uint32_t d = (key >> shift) & dmask;
+          atomicAdd(&h_cnt[d], 1u);
+          if (by_mass) atomicAdd(&h_mass[d], mass_of(v));
+        }
+      }
+      __syncthreads();
+      // thread t owns bins hi = 2047 - 2t and hi - 1; scan in descending bin order
+      const int hi = SMP_BINS - 1 - 2 * tid, lo = hi - 1;
+      const unsigned long long w_hi = by_mass ? h_mass[hi] : h_cnt[hi], w_lo = by_mass ? h_mass[lo] : h_cnt[lo];
+      unsigned long long tot;
+      const unsigned long long before_hi = above + block_exclusive_scan(w_hi + w_lo, s_u64, &tot);
+      const unsigned long long before_lo = before_hi + w_hi;
+      if (h_cnt[lo] > 0 && before_lo < limit) atomicMin(&s_bin, static_cast<uint32_t>(lo));
+      else if (h_cnt[hi] > 0 && before_hi < limit) atomicMin(&s_bin, static_cast<uint32_t>(hi));
+      __syncthreads();
+      const uint32_t sel = s_bin;
+      if (sel == static_cast<uint32_t>(lo)) s_above = before_lo;
+      if (sel == static_cast<uint32_t>(hi)) s_above = before_hi;
+      __syncthreads();
+      return sel;
+    };
+    // the cut key: radix descent over the three digits (bits 31..21, 20..10, 9..0)
+    auto select_key = [&](bool by_mass, unsigned long long limit) -> uint32_t {
+      uint32_t prefix = 0, himask = 0;
+      unsigned long long above = 0;
+#pragma unroll 1
+      for (int lvl = 0; lvl < 3; ++lvl) {
+        const int shift = lvl == 0 ? 21 : lvl == 1 ? 10 : 0;
+        const uint32_t d = radix_level(prefix, himask, shift, lvl == 2 ? 1023u : 2047u, by_mass, above, limit);
+        above = s_above;
+        prefix |= d << shift;
+        himask = lvl == 0 ? 0xFFE00000u : 0xFFFFFC00u;
+      }
+      return prefix;
+    };
+    auto kept_mass = [&]() -> unsigned long long {
+      unsigned long long m = 0, tot;
+      for (int i = tid; i < n; i += SMP_THREADS) {
+        const float v = srow[i];
+        if (order_key(v) >= thr) m += mass_of(v);
+      }
+      block_exclusive_scan(m, s_u64, &tot);
+      return tot;
+    };
+
+    // top-k: the k-th largest kept key; ties at it stay (count of strictly larger keys < k)
+    if (top_k > 0 && static_cast<uint32_t>(top_k) < valid) thr = select_key(false, static_cast<unsigned long long>(top_k));
+    unsigned long long total = kept_mass();
+    // top-p: keep i iff the kept mass of strictly larger keys is < top_p * total; the maximum always stays
+    if (top_p < 1.f) {
+      if (top_p <= 0.f) {
+        thr = order_key(mx);
+      } else {
+        const unsigned long long limit =
+            static_cast<unsigned long long>(ceil(static_cast<double>(top_p) * static_cast<double>(total)));
+        thr = select_key(true, limit);
+      }
+      total = kept_mass();
+    }
+
+    // draw: u = (philox[0] >> 8) * 2^-24; first kept index (vocabulary order) whose inclusive prefix mass > u * total.
+    // prefix > u * total  <=>  prefix > floor(a * total / 2^24) for integer prefix, a = philox[0] >> 8
+    const uint32_t t = (kv_len != nullptr && prompt_len != nullptr) ? static_cast<uint32_t>(kv_len[b] - prompt_len[b]) : 0u;
+    const unsigned long long seed = prm->seed;
+    const uint4 r = philox4x32_10(make_uint4(t, static_cast<uint32_t>(b), 0u, 0u), static_cast<uint32_t>(seed),
+                                  static_cast<uint32_t>(seed >> 32));
+    const unsigned long long a = r.x >> 8;
+    const unsigned long long target = (__umul64hi(a, total) << 40) | ((a * total) >> 24);
+    // thread t owns the contiguous chunk [t*C, t*C + C); the chunk sum is read rotated by t (conflict-free banks)
+    const int C = (n + SMP_THREADS - 1) / SMP_THREADS;
+    const int c0 = tid * C, c1 = min(n, c0 + C);
+    unsigned long long m = 0;
+    for (int j = 0; j < C; ++j) {
+      const int i = c0 + (j + tid) % C;
+      if (i < c1) {
+        const float v = srow[i];
+        if (order_key(v) >= thr) m += mass_of(v);
+      }
+    }
+    unsigned long long tot;
+    const unsigned long long before = block_exclusive_scan(m, s_u64, &tot);
+    if (before <= target && target < before + m) {   // exactly one thread: target < total, the chunks partition it
+      unsigned long long run = before;
+      for (int i = c0; i < c1; ++i) {
+        const float v = srow[i];
+        if (order_key(v) < thr) continue;
+        run += mass_of(v);
+        if (run > target) { s_tok = i; break; }
+      }
+    }
+    __syncthreads();
+    tok = s_tok;
+  }
+
+  if (tid == 0) {
+    if (out_idx) out_idx[b] = tok;
+    if (next_src) next_src[b] = tok;
+    if (token_log) {
+      const int step = kv_len[b] - prompt_len[b];  // tokens generated before this one
+      if (step >= 0 && step < log_stride) token_log[static_cast<long long>(b) * log_stride + step] = tok;
+    }
+    if (positions) positions[b] += 1;
+    if (kv_len) kv_len[b] += 1;
+  }
+}
+
 }  // namespace vb
 
 using namespace vb;
@@ -446,6 +688,29 @@ extern "C" int vb200_argmax_advance(const float* logits, int64_t ld, int64_t row
   cudaError_t e = vb_launch(argmax_advance_kernel, dim3(static_cast<unsigned>(rows)), dim3(1024), 0, stream, logits,
                             static_cast<long long>(ld), static_cast<int>(n), out_idx, next_src, positions, kv_len,
                             token_log, static_cast<int>(log_stride), prompt_len);
+  if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
+  return VB_OK;
+}
+
+extern "C" int vb200_sample_advance(const float* logits, int64_t ld, int64_t rows, int64_t n,
+                                    const vb_sample_params* params, int64_t* out_idx, int32_t* next_src,
+                                    int32_t* positions, int32_t* kv_len, int64_t* token_log, int64_t log_stride,
+                                    const int32_t* prompt_len, cudaStream_t stream) {
+  VB_CHECK_ARG(logits && params && rows > 0 && rows <= INT_MAX && n > 0 && ld >= n);
+  VB_CHECK_ARG(token_log == nullptr ||
+               (kv_len != nullptr && prompt_len != nullptr && log_stride > 0 && log_stride <= INT_MAX));
+  if (n > SMP_MAX_N) return VB_ERR_UNSUPPORTED;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(sample_advance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         SMP_MAX_N * static_cast<int>(sizeof(float)));
+    if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
+    attr_set = true;
+  }
+  cudaError_t e = vb_launch(sample_advance_kernel, dim3(static_cast<unsigned>(rows)), dim3(SMP_THREADS),
+                            static_cast<size_t>(n) * sizeof(float), stream, logits, static_cast<long long>(ld),
+                            static_cast<int>(n), params, out_idx, next_src, positions, kv_len, token_log,
+                            static_cast<int>(log_stride), prompt_len);
   if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
   return VB_OK;
 }

@@ -9,14 +9,14 @@ sequence is restated in-tree at vitron/train/llama_flash_attn_monkey_patch.py:30
 
 Differences in mechanism (not in math): q/k/v and gate/up are single fused GEMMs (weights packed
 at load), the KV cache is paged in HBM instead of grown with torch.cat, residual adds / SiLU*mul
-live in GEMM epilogues, and the decode step is one CUDA graph with the arg-max on device.
+live in GEMM epilogues, and the decode step is one CUDA graph with the arg-max (or the sampler) on device.
 State-dict names are the reference's (SURVEY.md Appendix B).
 """
 from dataclasses import dataclass
 
 import torch
 
-from . import ops
+from . import ops, sampling
 
 BF16 = torch.bfloat16
 
@@ -124,6 +124,8 @@ class LlamaEngine:
         # generated ids land here (column = tokens generated so far); persistent so the decode
         # graph survives across generate() calls
         self.token_log = torch.zeros((B, self.cache.max_seq_len), dtype=torch.int64, device=dev)
+        # vb_sample_params read by the sampled step: one captured graph serves every temperature / top-k / top-p / seed
+        self.d_sample = torch.zeros((ops.SAMPLE_PARAMS.size,), dtype=torch.uint8, device=dev)
         self._graphs = {}
         self.launches_per_step = 0
         self.use_pdl = True
@@ -307,20 +309,38 @@ class LlamaEngine:
                         max_kv_len=self.cache.max_seq_len)
         ops.gemm(h, self.lm_head, out=self.d_logits[:B], out_fp32=True, rms_eps=c.rms_norm_eps)
 
-    def _step_kernels(self, B):
+    def _step_kernels(self, B, sampled=False):
         from . import _lib
         lib = _lib.load()
         prev = lib.vb200_set_pdl(1 if self.use_pdl else 0)  # decode-step kernels overlap via PDL
         try:
-            self._step_kernels_inner(B)
+            self._step_kernels_inner(B, sampled)
         finally:
             lib.vb200_set_pdl(prev)
 
-    def _step_kernels_inner(self, B):
+    def _step_kernels_inner(self, B, sampled=False):
         self._decode_body(B)
-        # token_log[b, d_len - d_prompt] = arg-max; d_src = arg-max; d_pos += 1; d_len += 1
-        ops.argmax_advance(self.d_logits[:B], self.d_next[:B], next_src=self.d_src[:B], positions=self.d_pos[:B],
-                           kv_len=self.d_len[:B], token_log=self.token_log[:B], prompt_len=self.d_prompt[:B])
+        # token_log[b, d_len - d_prompt] = token; d_src = token; d_pos += 1; d_len += 1
+        state = dict(next_src=self.d_src[:B], positions=self.d_pos[:B], kv_len=self.d_len[:B], token_log=self.token_log[:B],
+                     prompt_len=self.d_prompt[:B])
+        if sampled:
+            self.sample_advance(self.d_logits[:B], self.d_next[:B], **state)
+        else:
+            ops.argmax_advance(self.d_logits[:B], self.d_next[:B], **state)
+
+    def sample_advance(self, logits, out_idx=None, **state):
+        """Sample rows of fp32 logits with the set_sampling parameters (ops.sample_advance arguments after `params`).
+        A CUDA engine runs the kernel; a CPU engine, which runs no kernels of this library, runs the host statement of
+        the same contract (vitron_b200.sampling)."""
+        fn = ops.sample_advance if self.device.type == "cuda" else sampling.sample_advance
+        return fn(logits, self.d_sample, out_idx, **state)
+
+    def set_sampling(self, temperature=1.0, top_k=None, top_p=None, seed=0):
+        """Parameters of the sampled decode step (read from self.d_sample): temperature clamped to >= 1e-6,
+        top_k None / 0 = off, top_p None = off, 64-bit Philox seed."""
+        k = 0 if not top_k or top_k < 0 else min(int(top_k), 2 ** 31 - 1)
+        p = 1.0 if top_p is None else float(top_p)
+        self.d_sample.copy_(ops.sample_params(max(float(temperature), 1e-6), k, p, seed))
 
     def start_decode(self, first_tokens, max_new_tokens):
         """first_tokens [B] int64: the token chosen from the prefill logits (already counted as
@@ -338,21 +358,22 @@ class LlamaEngine:
         self.token_log[:B, 0] = first_tokens
         self.d_src[:B] = first_tokens.to(torch.int32)
 
-    def decode_steps(self, B, n, use_graph=True):
-        """Run n greedy decode steps for slots 0..B-1 (no host sync)."""
+    def decode_steps(self, B, n, use_graph=True, sampled=False):
+        """Run n decode steps for slots 0..B-1 (no host sync): greedy, or sampled with the set_sampling parameters."""
         if n <= 0:
             return
         if not use_graph or self.device.type != "cuda":   # (host-logic tests drive the same step un-graphed)
             for _ in range(n):
-                self._step_kernels(B)
+                self._step_kernels(B, sampled)
             return
-        if B not in self._graphs:
+        key = (B, bool(sampled))
+        if key not in self._graphs:
             # warm-up on a side stream (allocator + lazy init), then capture
             s = torch.cuda.Stream(device=self.device)
             s.wait_stream(torch.cuda.current_stream())
             saved = [t.clone() for t in (self.d_src, self.d_pos, self.d_len, self.token_log)]
             with torch.cuda.stream(s):
-                self._step_kernels(B)
+                self._step_kernels(B, sampled)
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
             for t, sv in zip((self.d_src, self.d_pos, self.d_len, self.token_log), saved):
@@ -360,18 +381,18 @@ class LlamaEngine:
             g = torch.cuda.CUDAGraph()
             l0 = ops.launch_count()
             with torch.cuda.graph(g):
-                self._step_kernels(B)
+                self._step_kernels(B, sampled)
             self.launches_per_step = ops.launch_count() - l0
             for t, sv in zip((self.d_src, self.d_pos, self.d_len, self.token_log), saved):
                 t.copy_(sv)
-            self._graphs[B] = g
-        g = self._graphs[B]
+            self._graphs[key] = g
+        g = self._graphs[key]
         for _ in range(n):
             g.replay()
         ops.count_launches(n * self.launches_per_step)
 
     def decode_one_logits(self, tokens):
-        """Non-greedy path: feed tokens [B] and return fp32 logits [B, V] (sampling done by caller)."""
+        """Teacher forcing: feed tokens [B] and return fp32 logits [B, V] (the next token is the caller's choice)."""
         B = tokens.shape[0]
         self.d_src[:B] = tokens.to(torch.int32)
         self._decode_body(B)

@@ -5,6 +5,7 @@ hand-written CUDA kernels from libvitron_b200.so on the current torch stream. No
 """
 import ctypes as C
 import math
+import struct
 
 import torch
 
@@ -489,6 +490,35 @@ def argmax_advance(logits, out_idx, next_src=None, positions=None, kv_len=None, 
                                    out_idx.data_ptr(), _ptr(next_src), _ptr(positions), _ptr(kv_len),
                                    _ptr(token_log), token_log.shape[1] if token_log is not None else 0,
                                    _ptr(prompt_len), _stream()), "vb200_argmax_advance")
+    _launches[0] += 1
+    return out_idx
+
+
+SAMPLE_PARAMS = struct.Struct("<fifIQ")   # vb_sample_params: temperature, top_k, top_p, reserved, seed
+
+
+def sample_params(temperature, top_k, top_p, seed):
+    """vb_sample_params packed into a CPU uint8 tensor (copy it into the device buffer vb200_sample_advance reads).
+    top_k 0 = off, top_p >= 1 = off; the temperature is used as given."""
+    raw = SAMPLE_PARAMS.pack(float(temperature), int(top_k), float(top_p), 0, int(seed) & (2 ** 64 - 1))
+    return torch.frombuffer(bytearray(raw), dtype=torch.uint8)
+
+
+def sample_advance(logits, params, out_idx=None, next_src=None, positions=None, kv_len=None, token_log=None,
+                   prompt_len=None):
+    """Sampled sibling of argmax_advance: temperature, top-k, top-p and a Philox draw per row (contract in
+    include/vitron_b200.h), parameters read from the device buffer `params` (sample_params). Without kv_len /
+    prompt_len the draw is step 0 and no state advances (the token of the prefill logits)."""
+    lib = _lib.load()
+    _req(logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1, "fp32 logits [B, V]")
+    _req(params.dtype == torch.uint8 and params.numel() == SAMPLE_PARAMS.size and params.is_contiguous()
+         and params.device == logits.device, "params: uint8 [24] sampling buffer on the logits' device")
+    if out_idx is None:
+        out_idx = torch.empty((logits.shape[0],), dtype=torch.int64, device=logits.device)
+    check(lib.vb200_sample_advance(logits.data_ptr(), logits.stride(0), logits.shape[0], logits.shape[1],
+                                   params.data_ptr(), out_idx.data_ptr(), _ptr(next_src), _ptr(positions), _ptr(kv_len),
+                                   _ptr(token_log), token_log.shape[1] if token_log is not None else 0,
+                                   _ptr(prompt_len), _stream()), "vb200_sample_advance")
     _launches[0] += 1
     return out_idx
 

@@ -8,7 +8,7 @@ padding rules, and the reference's parameter names for `load_state_dict`.
 
 Mechanism: the per-sample Python cat/split loop becomes one host-side layout pass over the (tiny)
 id tensor plus a single gather kernel; the decoder runs on `LlamaEngine` (paged KV cache, fused
-kernels, CUDA-graph decode, arg-max on device).
+kernels, CUDA-graph decode, arg-max or sampler on device).
 """
 from types import SimpleNamespace
 
@@ -390,7 +390,11 @@ class VitronLlamaForCausalLM(ModuleFace):
                  eos_token_id=None, pad_token_id=None, inputs=None, sync_every=16, **kwargs):
         """Greedy (or sampled) decoding with the reference call signature
         (inference_image.py:53-61, app.py:562-571). Returns input_ids followed by the generated ids,
-        like HF `generate` for decoder-only models."""
+        like HF `generate` for decoder-only models.
+
+        Both modes replay the same CUDA-graphed decode step; do_sample=True ends it with the device sampler
+        (temperature, top_k, top_p, Philox draw) instead of the arg-max. Its seed is drawn once per call from torch's
+        default CPU generator, so `torch.manual_seed(s)` makes a sampled call reproducible."""
         if input_ids is None:
             input_ids = inputs
         eos = self.config.eos_token_id if eos_token_id is None else eos_token_id
@@ -408,9 +412,11 @@ class VitronLlamaForCausalLM(ModuleFace):
         eng = self.engine
         logits = eng.prefill(embeds, lens)
         if do_sample:
-            return self._sample_loop(input_ids, logits, B, max_new_tokens, temperature, top_p, top_k, eos_set, pad,
-                                     stopping_criteria)
-        first = ops.argmax_rows(logits)
+            seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64)) & (2 ** 64 - 1)
+            eng.set_sampling(temperature, top_k, top_p, seed)
+            first = eng.sample_advance(logits)                        # generated token 0: Philox step 0
+        else:
+            first = ops.argmax_rows(logits)
         eng.start_decode(first, max_new_tokens)
         done_at = [None] * B  # index of the last kept token per sequence
         produced = 1
@@ -433,7 +439,7 @@ class VitronLlamaForCausalLM(ModuleFace):
             if stop_all is not None or all(d is not None for d in done_at) or produced >= max_new_tokens:
                 break
             n = min(sync_every, max_new_tokens - produced)
-            eng.decode_steps(B, n)
+            eng.decode_steps(B, n, sampled=do_sample)
             produced += n
         keep = produced if stop_all is None else stop_all
         if all(d is not None for d in done_at):
@@ -459,35 +465,6 @@ class VitronLlamaForCausalLM(ModuleFace):
         if isinstance(r, torch.Tensor):
             return bool(r.all())
         return bool(r)
-
-    def _sample_loop(self, input_ids, logits, B, max_new_tokens, temperature, top_p, top_k, eos_set, pad, criteria):
-        eng = self.engine
-        out = []
-        finished = torch.zeros(B, dtype=torch.bool, device=logits.device)
-        for step in range(max_new_tokens):
-            lg = logits.float() / max(float(temperature), 1e-6)
-            if top_k:
-                kth = torch.topk(lg, int(top_k), dim=-1).values[:, -1:]
-                lg = lg.masked_fill(lg < kth, float("-inf"))
-            if top_p is not None and top_p < 1.0:
-                sl, si = torch.sort(lg, descending=True, dim=-1)
-                cp = torch.softmax(sl, -1).cumsum(-1)
-                rm = cp - torch.softmax(sl, -1) > top_p
-                sl = sl.masked_fill(rm, float("-inf"))
-                lg = torch.full_like(lg, float("-inf")).scatter(1, si, sl)
-            tok = torch.multinomial(torch.softmax(lg, -1), 1).squeeze(1)
-            tok = torch.where(finished, torch.full_like(tok, pad), tok)
-            out.append(tok)
-            for e in eos_set:
-                finished |= tok == e
-            seq = torch.cat([input_ids, torch.stack(out, 1).to(input_ids.device)], 1)
-            if bool(finished.all()) or (criteria is not None and self._criteria_met(criteria, seq)):
-                break
-            if step == 0:
-                eng.start_decode(tok, max_new_tokens)
-            if step + 1 < max_new_tokens:
-                logits = eng.decode_one_logits(tok)
-        return torch.cat([input_ids, torch.stack(out, 1).to(input_ids.device)], 1)
 
 
 LlavaLlamaForCausalLM = VitronLlamaForCausalLM  # the reference's class name
