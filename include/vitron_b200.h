@@ -89,6 +89,25 @@ int vb200_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void
                     int64_t M, int64_t N, int64_t K, const vb_epilogue* epi, void* workspace,
                     size_t workspace_bytes, cudaStream_t stream);
 
+/* ---- NF4 weights (gemv_nf4.cu; format stated in vitron_b200/nf4.py) --------------------------
+ * The reference's `load_pretrained_model(..., load_4bit=True)` (vitron/model/builder.py:36-46) loads the LLM through
+ * bitsandbytes as NF4 with double-quantised block scales. Here a weight W_eff[N, K] (K % 64 == 0) is
+ *   codes:  uint8 [N, ceil(K/128) * 64], 4-bit codes into bitsandbytes' nf4 table, in the kernel's byte order (nf4.py
+ *           pack_codes); the row stride is implied by K;
+ *   scales: fp16 [N, K / 64], one scale per (row, 64-column block): W_eff[n, k] = nf4[code] * float(scale[n, k / 64]).
+ * vb200_gemm_nf4: out = epi(rowscale ⊙ (A · diag(kscale) · W_effᵀ)) with every vb_epilogue feature of vb200_gemm_bf16
+ * (rms_eps computes the row scale from the raw A), for M <= 32 (else VB_ERR_UNSUPPORTED); kscale is an optional fp32
+ * [K] column scale (16-byte aligned) applied to A in fp32 and rounded to bf16 before the products, which is how the
+ * RMSNorm gain reaches a weight that was quantised unfolded. One launch, no workspace. lda multiple of 8.
+ * vb200_nf4_dequant: out[N, K] bf16 (contiguous, 16-byte aligned) = bf16_rn((nf4[code] * scale) * kscale[k]), fp32
+ * products in that order (kscale NULL = 1), bit-identical to nf4.py; larger M runs it into a workspace and then
+ * vb200_gemm_bf16. Both follow the PDL rule of vb200_gemm_bf16's weight operand: codes, scales and kscale are
+ * requested before the dependency wait and must be constants. */
+int vb200_gemm_nf4(const void* A, int64_t lda, const void* codes, const void* scales, const float* kscale, void* out,
+                   int64_t ldo, int64_t M, int64_t N, int64_t K, const vb_epilogue* epi, cudaStream_t stream);
+int vb200_nf4_dequant(const void* codes, const void* scales, const float* kscale, void* out, int64_t N, int64_t K,
+                      cudaStream_t stream);
+
 
 
 /* ---- implicit-GEMM convolution on NHWC activations, im2col-free (gemm.cu) ----------------

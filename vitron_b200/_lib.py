@@ -37,6 +37,8 @@ SIGNATURES = {
     "vb200_attention_tc_occupancy": (_i32, [_i32]),
     "vb200_gemm_bf16_workspace_size": (_sz, [_i64, _i64, _i64]),
     "vb200_gemm_bf16": (_i32, [_p, _i64, _p, _i64, _p, _i64, _i64, _i64, _i64, C.POINTER(Epilogue), _p, _sz, _p]),
+    "vb200_gemm_nf4": (_i32, [_p, _i64, _p, _p, _p, _p, _i64, _i64, _i64, _i64, C.POINTER(Epilogue), _p]),
+    "vb200_nf4_dequant": (_i32, [_p, _p, _p, _p, _i64, _i64, _p]),
     "vb200_conv_nhwc_workspace_size": (_sz, [_i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32]),
     "vb200_conv_nhwc_bf16": (_i32, [_p, _p, _p, _i64, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32,
                                     C.POINTER(Epilogue), _p, _sz, _p]),

@@ -9,9 +9,25 @@ import re
 
 import torch
 
+from . import nf4 as _nf4
 from . import ops
 
 BF16 = torch.bfloat16
+
+
+def _linear_weight(w, nf4):
+    """bf16 weight, or with nf4 (the reference's load_4bit, whose replace_with_bnb_linear converts every Linear these
+    modules hold) an NF4Weight; a Linear whose input width is not a multiple of 64 (the 4-input location encoder) stays
+    bf16, the one place where the NF4 format of vitron_b200.nf4 does not reach."""
+    return _nf4.quantize(w) if nf4 and w.shape[1] % _nf4.BLOCK == 0 else w
+
+
+def _dense(w):
+    return _nf4.dequantize(w).to(BF16) if isinstance(w, _nf4.NF4Weight) else w
+
+
+def _tensors(w):
+    return (w.codes, w.scales) if isinstance(w, _nf4.NF4Weight) else (w,)
 
 
 class VisionProjector:
@@ -30,26 +46,28 @@ class VisionProjector:
             self.depth = int(m.group(1))
         self.mm_hidden_size, self.hidden_size = mm_hidden_size, hidden_size
 
-    def load_state_dict(self, sd, prefix=""):
-        """names: '<prefix>weight/bias' (linear) or '<prefix>{0,2,4..}.weight/bias' (mlpNx_gelu)."""
+    def load_state_dict(self, sd, prefix="", nf4=False):
+        """names: '<prefix>weight/bias' (linear) or '<prefix>{0,2,4..}.weight/bias' (mlpNx_gelu). nf4: weights in NF4,
+        biases bf16."""
         get = lambda n: sd[prefix + n].detach().to(device=self.device, dtype=BF16).contiguous()
+        w = lambda n: _linear_weight(get(n), nf4)
         if self.projector_type == "linear":
-            self.linears = [(get("weight"), get("bias"))]
+            self.linears = [(w("weight"), get("bias"))]
         else:
-            self.linears = [(get(f"{2 * i}.weight"), get(f"{2 * i}.bias")) for i in range(self.depth)]
+            self.linears = [(w(f"{2 * i}.weight"), get(f"{2 * i}.bias")) for i in range(self.depth)]
         return self
 
     def state_dict(self, prefix=""):
         if self.projector_type == "linear":
-            return {prefix + "weight": self.linears[0][0], prefix + "bias": self.linears[0][1]}
+            return {prefix + "weight": _dense(self.linears[0][0]), prefix + "bias": self.linears[0][1]}
         out = {}
         for i, (w, b) in enumerate(self.linears):
-            out[f"{prefix}{2 * i}.weight"], out[f"{prefix}{2 * i}.bias"] = w, b
+            out[f"{prefix}{2 * i}.weight"], out[f"{prefix}{2 * i}.bias"] = _dense(w), b
         return out
 
     def parameters(self):
         for w, b in self.linears:
-            yield w
+            yield from _tensors(w)
             yield b
 
     def __call__(self, x):
@@ -83,29 +101,32 @@ class RegionExtractor:
         self.mlp = []
         self.loc = []
 
-    def load_state_dict(self, sd, prefix=""):
-        """names: region_linear.layers.{0,1,2}.{weight,bias}, loc_encoder.loc_encoder.{0,2}.{weight,bias}."""
+    def load_state_dict(self, sd, prefix="", nf4=False):
+        """names: region_linear.layers.{0,1,2}.{weight,bias}, loc_encoder.loc_encoder.{0,2}.{weight,bias}. nf4: weights
+        in NF4 (except the 4-input location layer), biases bf16."""
         get = lambda n: sd[prefix + n].detach().to(device=self.device, dtype=BF16).contiguous()
-        self.mlp = [(get(f"region_linear.layers.{i}.weight"), get(f"region_linear.layers.{i}.bias")) for i in range(3)]
+        self.mlp = [(_linear_weight(get(f"region_linear.layers.{i}.weight"), nf4), get(f"region_linear.layers.{i}.bias"))
+                    for i in range(3)]
         w0 = get("loc_encoder.loc_encoder.0.weight")  # [hidden/2, 4] -> pad K to 8 for 16-byte rows
         w0p = torch.zeros((w0.shape[0], 8), dtype=BF16, device=self.device)
         w0p[:, :4] = w0
         self.loc = [(w0p, get("loc_encoder.loc_encoder.0.bias")),
-                    (get("loc_encoder.loc_encoder.2.weight"), get("loc_encoder.loc_encoder.2.bias"))]
+                    (_linear_weight(get("loc_encoder.loc_encoder.2.weight"), nf4), get("loc_encoder.loc_encoder.2.bias"))]
         return self
 
     def state_dict(self, prefix=""):
         out = {}
         for i, (w, b) in enumerate(self.mlp):
-            out[f"{prefix}region_linear.layers.{i}.weight"], out[f"{prefix}region_linear.layers.{i}.bias"] = w, b
+            out[f"{prefix}region_linear.layers.{i}.weight"], out[f"{prefix}region_linear.layers.{i}.bias"] = _dense(w), b
         out[prefix + "loc_encoder.loc_encoder.0.weight"] = self.loc[0][0][:, :4].contiguous()
         out[prefix + "loc_encoder.loc_encoder.0.bias"] = self.loc[0][1]
-        out[prefix + "loc_encoder.loc_encoder.2.weight"], out[prefix + "loc_encoder.loc_encoder.2.bias"] = self.loc[1]
+        out[prefix + "loc_encoder.loc_encoder.2.weight"] = _dense(self.loc[1][0])
+        out[prefix + "loc_encoder.loc_encoder.2.bias"] = self.loc[1][1]
         return out
 
     def parameters(self):
         for w, b in self.mlp + self.loc:
-            yield w
+            yield from _tensors(w)
             yield b
 
     def forward(self, feats, regions):

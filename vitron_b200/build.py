@@ -14,7 +14,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libvitron_b200.so")
-SOURCES = ["core.cu", "gemm.cu", "gemm_v2_bn256.cu", "gemm_v2_bn160.cu", "gemm_v2_bn128.cu", "gemm_v2_bn64.cu", "gemm_v2_bn32.cu", "gemm_v2_resb.cu", "gemv.cu", "norm.cu", "attention.cu", "attention_tc.cu", "llm.cu", "vision.cu", "focal.cu", "preprocess.cu"]
+SOURCES = ["core.cu", "gemm.cu", "gemm_v2_bn256.cu", "gemm_v2_bn160.cu", "gemm_v2_bn128.cu", "gemm_v2_bn64.cu", "gemm_v2_bn32.cu", "gemm_v2_resb.cu", "gemv.cu", "gemv_nf4.cu", "norm.cu", "attention.cu", "attention_tc.cu", "llm.cu", "vision.cu", "focal.cu", "preprocess.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC,

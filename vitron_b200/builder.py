@@ -16,7 +16,12 @@ read a checkpoint directory):
     W += (lora_B @ lora_A) * lora_alpha / r  — the arithmetic of `PeftModel.merge_and_unload()` (:83-84);
   * projector-only checkpoint (`model_base` given, no 'lora', builder.py:85-103): base weights + `mm_projector.bin`;
   * special tokens added to the tokenizer and the embeddings resized (builder.py:139-146);
-  * 8-bit / 4-bit loading (bitsandbytes, :36-46) is not offered: the path computes in bf16 — a request raises ValueError.
+  * 4-bit loading (`load_4bit=True`, bitsandbytes NF4 with double-quantised scales, :36-46): the language model's
+    projections, the mm_projector and the region extractor are quantised with vitron_b200.nf4 and served by the NF4
+    kernels; embed_tokens, lm_head and the vision towers stay bf16. A LoRA is merged in float BEFORE quantisation (the
+    reference runs it through peft on the quantised base instead);
+  * 8-bit loading (LLM.int8, whose outlier decomposition depends on the activations) is not offered: a request raises
+    ValueError.
 `cache_dir`, `device_map`, `torch_dtype` keywords are accepted and ignored like any other `from_pretrained` keyword the
 CUDA path has no use for. Extra keywords: `tokenizer=` (a ready tokenizer object instead of `AutoTokenizer.from_pretrained`),
 `max_batch=` / `max_seq_len=` (KV-cache capacity of the engine; default 8 x context_len)."""
@@ -124,8 +129,8 @@ def _vision_cfg(cfg, key, cache_dir, video):
 
 def load_pretrained_model(model_path, model_base, model_name, load_8bit=False, load_4bit=False, device_map="auto", device="cuda",
                           **kwargs):
-    if load_8bit or load_4bit:
-        raise ValueError("vitron_b200 computes in bf16: bitsandbytes 8-bit / 4-bit loading (builder.py:36-46) is not offered")
+    if load_8bit:
+        raise ValueError("vitron_b200 does not offer 8-bit loading (LLM.int8, builder.py:36-39); load_4bit=True serves NF4")
     cache_dir = kwargs.pop("cache_dir", None)
     tokenizer = kwargs.pop("tokenizer", None)
     max_batch = int(kwargs.pop("max_batch", 8))
@@ -178,7 +183,7 @@ def load_pretrained_model(model_path, model_base, model_name, load_8bit=False, l
                         mm_use_im_patch_token=cfg.get("mm_use_im_patch_token", True), max_sequence_length=context_len)
     model = VitronLlamaForCausalLM(vcfg, dev, max_batch=max_batch, max_seq_len=int(kwargs.pop("max_seq_len", context_len)))
     # towers whose weights are not inside the checkpoint are left unloaded exactly like `is_loaded == False` in the reference
-    model.load_state_dict(sd)
+    model.load_state_dict(sd, nf4=bool(load_4bit))
     del sd
 
     processor = {"image": None, "video": None}

@@ -16,6 +16,7 @@ from dataclasses import dataclass
 
 import torch
 
+from . import nf4 as _nf4
 from . import ops, sampling
 
 BF16 = torch.bfloat16
@@ -135,10 +136,17 @@ class LlamaEngine:
             ops.reserve_decode_workspace(max_batch, c.num_attention_heads, c.head_dim, self.device)
 
     # ------------------------------------------------------------------ weights
-    def load_state_dict(self, sd, prefix=""):
+    def load_state_dict(self, sd, prefix="", nf4=False):
         """HF names: model.embed_tokens.weight, model.layers.N.self_attn.{q,k,v,o}_proj.weight,
         model.layers.N.mlp.{gate,up,down}_proj.weight, model.layers.N.{input,post_attention}_layernorm.weight,
-        model.norm.weight, lm_head.weight."""
+        model.norm.weight, lm_head.weight.
+
+        nf4=True is the reference's load_4bit (builder.py:36-46): the seven projections of every layer are quantised to NF4
+        (vitron_b200.nf4) from the checkpoint tensors, one tensor at a time on the load device; the RMSNorm gains cannot be
+        folded into quantised weights and are applied as the kernels' column scale instead. embed_tokens and lm_head stay
+        bf16, as bitsandbytes leaves them."""
+        if nf4:
+            return self._load_nf4(sd, prefix)
         dev = self.device
 
         def get(name):
@@ -169,22 +177,64 @@ class LlamaEngine:
         self._graphs = {}
         return self
 
-    def init_random(self, seed=0, std=0.02):
-        """Random-init weights of the configured architecture directly on the device (benchmarks)."""
+    def _load_nf4(self, sd, prefix):
+        dev = self.device
+        t = lambda n: sd[prefix + n].detach().to(device=dev)
+        g32 = lambda n: t(n).to(torch.float32).contiguous()
+        q = lambda n: _nf4.quantize(t(n))
+        self.embed = t("model.embed_tokens.weight").to(BF16).contiguous()
+        gn = g32("model.norm.weight")
+        self.lm_head = (t("lm_head.weight").to(torch.float32) * gn[None, :]).to(BF16).contiguous()
+        self.norm_gains = dict(norm=gn, ln1=[], ln2=[])
+        self.layers = []
+        for i in range(self.cfg.num_hidden_layers):
+            p = f"model.layers.{i}."
+            g1, g2 = g32(p + "input_layernorm.weight"), g32(p + "post_attention_layernorm.weight")
+            self.norm_gains["ln1"].append(g1)
+            self.norm_gains["ln2"].append(g2)
+            wqkv = _nf4.NF4Weight.cat([q(p + "self_attn.q_proj.weight"), q(p + "self_attn.k_proj.weight"),
+                                       q(p + "self_attn.v_proj.weight")])
+            self.layers.append(dict(wqkv=wqkv, wo=q(p + "self_attn.o_proj.weight"),
+                                    wgu=_pack_glu_nf4(q(p + "mlp.gate_proj.weight"), q(p + "mlp.up_proj.weight")),
+                                    wdown=q(p + "mlp.down_proj.weight"), g1=g1, g2=g2))
+        self._nf4_ready()
+        return self
+
+    def _nf4_ready(self):
+        self._graphs = {}
+        # decode at batch > NF4_MAX_M dequantises into a workspace whose address a captured graph keeps: size it now
+        if self.device.type == "cuda" and self.max_batch > ops.NF4_MAX_M:
+            ops.reserve_nf4_workspace([w for L in self.layers for w in (L["wqkv"], L["wo"], L["wgu"], L["wdown"])],
+                                      self.device)
+
+    @property
+    def nf4(self):
+        return bool(self.layers) and isinstance(self.layers[0]["wqkv"], _nf4.NF4Weight)
+
+    def init_random(self, seed=0, std=0.02, nf4=False):
+        """Random-init weights of the configured architecture directly on the device (benchmarks); nf4=True quantises
+        the projections as load_state_dict(nf4=True) does (unit RMSNorm gains, applied as the column scale)."""
         c, dev = self.cfg, self.device
         g = torch.Generator(device=dev).manual_seed(seed)
 
         def w(*shape):
-            return (torch.randn(shape, generator=g, device=dev, dtype=torch.float32) * std).to(BF16)
+            v = (torch.randn(shape, generator=g, device=dev, dtype=torch.float32) * std).to(BF16)
+            return _nf4.quantize(v) if nf4 and len(shape) == 2 and shape != (c.vocab_size, c.hidden_size) else v
 
         self.embed = w(c.vocab_size, c.hidden_size)
         self.lm_head = w(c.vocab_size, c.hidden_size)  # unit RMSNorm gains: folding is the identity
         self.layers = []
+        ones = torch.ones((c.hidden_size,), dtype=torch.float32, device=dev)
         for _ in range(c.num_hidden_layers):
-            self.layers.append(dict(
-                wqkv=w(3 * c.hidden_size, c.hidden_size), wo=w(c.hidden_size, c.hidden_size),
-                wgu=ops.pack_glu_weight(w(c.intermediate_size, c.hidden_size), w(c.intermediate_size, c.hidden_size)),
-                wdown=w(c.hidden_size, c.intermediate_size)))
+            gate, up = w(c.intermediate_size, c.hidden_size), w(c.intermediate_size, c.hidden_size)
+            L = dict(wqkv=w(3 * c.hidden_size, c.hidden_size), wo=w(c.hidden_size, c.hidden_size),
+                     wgu=_pack_glu_nf4(gate, up) if nf4 else ops.pack_glu_weight(gate, up),
+                     wdown=w(c.hidden_size, c.intermediate_size))
+            if nf4:
+                L.update(g1=ones, g2=ones)
+            self.layers.append(L)
+        if nf4:
+            self._nf4_ready()
         self._graphs = {}
         return self
 
@@ -196,8 +246,12 @@ class LlamaEngine:
         d, f = c.hidden_size, c.intermediate_size
         gains = getattr(self, "norm_gains", None)
         ones = torch.ones((d,), dtype=torch.float32, device=self.device)
+        nf4 = self.nf4
 
         def unfold(w, g):
+            # NF4 layers hold the unfolded W_eff (returned in bf16; bitsandbytes' packed-uint8 state dict is not reproduced)
+            if isinstance(w, _nf4.NF4Weight):
+                return _nf4.dequantize(w).to(BF16)
             return (w.float() / g[None, :]).to(BF16)
         out[prefix + "model.embed_tokens.weight"] = self.embed
         gn = gains["norm"] if gains else ones
@@ -207,14 +261,16 @@ class LlamaEngine:
             p = f"{prefix}model.layers.{i}."
             g1 = gains["ln1"][i] if gains else ones
             g2 = gains["ln2"][i] if gains else ones
-            q, k, v = L["wqkv"].split(d, 0)
+            q, k, v = (L["wqkv"].rows(j * d, (j + 1) * d) for j in range(3)) if nf4 else L["wqkv"].split(d, 0)
             out[p + "self_attn.q_proj.weight"], out[p + "self_attn.k_proj.weight"], out[p + "self_attn.v_proj.weight"] = \
                 unfold(q, g1), unfold(k, g1), unfold(v, g1)
-            out[p + "self_attn.o_proj.weight"] = L["wo"]
-            gu = L["wgu"].view(f // 16, 2, 16, d)      # ops.pack_glu_weight: 16-row blocks [gate | up]
-            out[p + "mlp.gate_proj.weight"] = unfold(gu[:, 0].reshape(f, d), g2)
-            out[p + "mlp.up_proj.weight"] = unfold(gu[:, 1].reshape(f, d), g2)
-            out[p + "mlp.down_proj.weight"] = L["wdown"]
+            dense = lambda w: _nf4.dequantize(w).to(BF16) if nf4 else w
+            out[p + "self_attn.o_proj.weight"] = dense(L["wo"])
+            wgu = _nf4.dequantize(L["wgu"]) if nf4 else L["wgu"]
+            gu = wgu.view(f // 16, 2, 16, d)           # ops.pack_glu_weight: 16-row blocks [gate | up]
+            out[p + "mlp.gate_proj.weight"] = unfold(gu[:, 0].reshape(f, d), ones if nf4 else g2)
+            out[p + "mlp.up_proj.weight"] = unfold(gu[:, 1].reshape(f, d), ones if nf4 else g2)
+            out[p + "mlp.down_proj.weight"] = dense(L["wdown"])
             out[p + "input_layernorm.weight"] = g1.to(BF16)
             out[p + "post_attention_layernorm.weight"] = g2.to(BF16)
         return out
@@ -223,13 +279,19 @@ class LlamaEngine:
         yield self.embed
         yield self.lm_head
         for L in self.layers:
-            yield from (L["wqkv"], L["wo"], L["wgu"], L["wdown"])
+            for w in (L["wqkv"], L["wo"], L["wgu"], L["wdown"]):
+                if isinstance(w, _nf4.NF4Weight):
+                    yield from (w.codes, w.scales)
+                else:
+                    yield w
 
     def weight_bytes(self):
-        n = self.lm_head.numel()
+        """Bytes of weights one decode step streams (lm_head and the layer projections; NF4 codes + scales as stored)."""
+        n = 2 * self.lm_head.numel()
         for l in self.layers:
-            n += l["wqkv"].numel() + l["wo"].numel() + l["wgu"].numel() + l["wdown"].numel()
-        return 2 * n
+            for w in (l["wqkv"], l["wo"], l["wgu"], l["wdown"]):
+                n += w.nbytes if isinstance(w, _nf4.NF4Weight) else 2 * w.numel()
+        return n
 
     # ------------------------------------------------------------------ layers
     def _layer(self, i, h, positions, bot, slots, prefill_shape=None, kv_len=None, max_kv_len=0):
@@ -238,7 +300,8 @@ class LlamaEngine:
         weight-streaming kernel for T <= 16)."""
         c, L, cache = self.cfg, self.layers[i], self.cache
         H, D = c.num_attention_heads, c.head_dim
-        qkv = ops.gemm(h, L["wqkv"], rms_eps=c.rms_norm_eps)
+        g1, g2 = L.get("g1"), L.get("g2")        # RMSNorm gains of NF4 layers (bf16 layers have them folded in)
+        qkv = ops.gemm(h, L["wqkv"], rms_eps=c.rms_norm_eps, **({} if g1 is None else dict(kscale=g1)))
         if prefill_shape is not None:
             B, S = prefill_shape
             ops.rope_kv_append(qkv, positions, H, D, c.rope_theta, cache.k(i), cache.v(i), cache.block_table, bot, slots,
@@ -250,7 +313,7 @@ class LlamaEngine:
             att = ops.attn_decode_rope(qkv, self._rope_tab, cache.k(i), cache.v(i), cache.block_table, kv_len, H, D,
                                        cache.page_size, max_kv_len)
         ops.gemm(att, L["wo"], residual=h, out=h)
-        act = ops.gemm(h, L["wgu"], glu=ops.GLU_SWIGLU, rms_eps=c.rms_norm_eps)
+        act = ops.gemm(h, L["wgu"], glu=ops.GLU_SWIGLU, rms_eps=c.rms_norm_eps, **({} if g2 is None else dict(kscale=g2)))
         ops.gemm(act, L["wdown"], residual=h, out=h)
         return h
 
@@ -399,3 +462,8 @@ class LlamaEngine:
         self.d_pos[:B].add_(1)
         self.d_len[:B].add_(1)
         return self.d_logits[:B]
+
+
+def _pack_glu_nf4(a, b):
+    """ops.pack_glu_weight's 16-row interleave applied to the rows of two NF4 weights."""
+    return _nf4.NF4Weight(ops.pack_glu_weight(a.codes, b.codes), ops.pack_glu_weight(a.scales, b.scales), a.k)

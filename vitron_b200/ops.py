@@ -10,6 +10,7 @@ import struct
 import torch
 
 from . import _lib
+from .nf4 import NF4Weight
 from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_RELU, ACT_SILU, GLU_GEGLU, GLU_NONE,
                    GLU_SWIGLU, Epilogue, check)
 
@@ -138,14 +139,20 @@ def pack_glu_weight(w_a, w_b):
 
 
 def gemm(a, w, bias=None, act=ACT_NONE, glu=GLU_NONE, residual=None, alpha=1.0, rowbias=None,
-         rowbias_rows=0, out=None, out_fp32=False, rowscale=None, rms_eps=0.0):
-    """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T) on wgmma tensor cores."""
+         rowbias_rows=0, out=None, out_fp32=False, rowscale=None, rms_eps=0.0, kscale=None):
+    """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T) on wgmma tensor cores. w is bf16, or an NF4Weight (nf4.py): then
+    out = epilogue(a @ diag(kscale) @ W_eff^T) with the optional fp32 column scale kscale [K], on the NF4 weight-streaming
+    kernel for M <= 32 and as an NF4 -> bf16 dequantisation into a workspace followed by the bf16 GEMM above that."""
     lib = _lib.load()
     a2, lda = _rows2d(a)
-    _req(a2.dtype == BF16 and w.dtype == BF16, "gemm operands must be bf16")
-    _req(w.dim() == 2 and w.stride(1) == 1 and w.shape[1] == a2.shape[1], "weight must be [N, K] row-major")
+    q4 = isinstance(w, NF4Weight)
+    _req(a2.dtype == BF16 and (q4 or w.dtype == BF16), "gemm operands must be bf16 (or an NF4Weight)")
+    _req(len(w.shape) == 2 and w.shape[1] == a2.shape[1] and (q4 or w.stride(1) == 1), "weight must be [N, K] row-major")
+    _req(kscale is None or (q4 and kscale.dtype == torch.float32 and kscale.is_contiguous()
+                            and kscale.numel() == a2.shape[1]), "kscale: fp32 [K], NF4 weights only")
     M, K = a2.shape
     N = w.shape[0]
+    small = M <= (NF4_MAX_M if q4 else 16)      # the weight-streaming kernels compute the RMS row scale themselves
     n_out = N // 2 if glu != GLU_NONE else N
     if out is None:
         out = torch.empty((M, n_out), dtype=torch.float32 if out_fp32 else BF16, device=a.device)
@@ -165,7 +172,7 @@ def gemm(a, w, bias=None, act=ACT_NONE, glu=GLU_NONE, residual=None, alpha=1.0, 
         _req(rowscale.dtype == torch.float32 and rowscale.numel() == M and rowscale.is_contiguous(), "bad rowscale")
         epi.rowscale = rowscale.data_ptr()
     elif rms_eps > 0:
-        if M <= 16:
+        if small:
             epi.rms_eps = float(rms_eps)  # computed inside the weight-streaming kernel
         else:
             rs = row_rstd(a2, rms_eps)
@@ -179,12 +186,45 @@ def gemm(a, w, bias=None, act=ACT_NONE, glu=GLU_NONE, residual=None, alpha=1.0, 
         _req(bias.dtype == BF16 and bias.numel() == N and bias.is_contiguous(), "bad bias")
     if M == 0:
         return out.reshape(*a.shape[:-1], n_out) if a.dim() != 2 else out
+    if q4 and small:
+        check(lib.vb200_gemm_nf4(a2.data_ptr(), lda, w.codes.data_ptr(), w.scales.data_ptr(), _ptr(kscale),
+                                 out2.data_ptr(), ldo, M, N, K, C.byref(epi), _stream()), "vb200_gemm_nf4")
+        _launches[0] += 1
+        return out.reshape(*a.shape[:-1], n_out) if a.dim() != 2 else out
+    if q4:
+        w = nf4_dequant(w, kscale, workspace(2 * N * K, a.device, "nf4"))
     need = lib.vb200_gemm_bf16_workspace_size(M, N, K)
     ws = workspace(need, a.device) if need else None
     check(lib.vb200_gemm_bf16(a2.data_ptr(), lda, w.data_ptr(), w.stride(0), out2.data_ptr(), ldo, M, N, K,
                               C.byref(epi), _ptr(ws), need, _stream()), "vb200_gemm_bf16")
     _launches[0] += 1
     return out.reshape(*a.shape[:-1], n_out) if a.dim() != 2 else out
+
+
+NF4_MAX_M = 32   # rows of A that vb200_gemm_nf4 takes; larger M dequantises into a workspace and runs the bf16 GEMM
+
+
+def nf4_dequant(w, kscale=None, out=None):
+    """bf16 [N, K] = bf16_rn((NF4[code] * scale) * kscale[k]) of an NF4Weight (bit-identical to nf4.dequantize).
+    out: a bf16 [N, K] tensor or a uint8 workspace of at least 2 N K bytes."""
+    N, K = w.shape
+    if out is None:
+        out = torch.empty((N, K), dtype=BF16, device=w.device)
+    else:
+        _req(out.is_contiguous() and out.numel() * out.element_size() >= 2 * N * K, "nf4_dequant: out too small")
+        out = out.view(torch.uint8)[:2 * N * K].view(BF16).view(N, K) if out.dtype != BF16 else out.view(N, K)
+    _req(kscale is None or (kscale.dtype == torch.float32 and kscale.is_contiguous() and kscale.numel() == K), "bad kscale")
+    check(_lib.load().vb200_nf4_dequant(w.codes.data_ptr(), w.scales.data_ptr(), _ptr(kscale), out.data_ptr(), N, K,
+                                        _stream()), "vb200_nf4_dequant")
+    _launches[0] += 1
+    return out
+
+
+def reserve_nf4_workspace(weights, device):
+    """Pre-size the dequantisation workspace for the largest of `weights` (NF4Weight), so that a CUDA graph captured at
+    M > NF4_MAX_M never sees the workspace move."""
+    need = max((2 * w.shape[0] * w.shape[1] for w in weights), default=0)
+    return workspace(need, torch.device(device), "nf4") if need else None
 
 
 def set_gemm_impl(impl):

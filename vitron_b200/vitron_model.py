@@ -223,16 +223,18 @@ class VitronLlamaForCausalLM(ModuleFace):
         self.config.vocab_size = new_num_tokens
         return self
 
-    def load_state_dict(self, sd, strict=True):
+    def load_state_dict(self, sd, strict=True, nf4=False):
         """Accepts the reference's names: model.embed_tokens.*, model.layers.*, lm_head.weight,
         model.mm_projector.*, model.region_extractor.*, model.image_tower.image_tower.*,
-        model.video_tower.video_tower.* (SURVEY.md Appendix B)."""
-        self.engine.load_state_dict(sd)
+        model.video_tower.video_tower.* (SURVEY.md Appendix B). nf4=True is the reference's load_4bit: the language
+        model's projections, the mm_projector and the region extractor's Linears are NF4 (vitron_b200.nf4; bitsandbytes
+        converts every Linear that LlavaMetaModel builds and skips only lm_head); the vision towers stay bf16."""
+        self.engine.load_state_dict(sd, nf4=nf4)
         m = self.model
         if m.mm_projector is not None and any(k.startswith("model.mm_projector.") for k in sd):
-            m.mm_projector.load_state_dict(sd, "model.mm_projector.")
+            m.mm_projector.load_state_dict(sd, "model.mm_projector.", nf4=nf4)
         if m.region_extractor is not None and any(k.startswith("model.region_extractor.") for k in sd):
-            m.region_extractor.load_state_dict(sd, "model.region_extractor.")
+            m.region_extractor.load_state_dict(sd, "model.region_extractor.", nf4=nf4)
         if m.image_tower is not None and any(k.startswith("model.image_tower.image_tower.") for k in sd):
             m.image_tower.vit.load_state_dict(sd, "model.image_tower.image_tower.")
         if m.video_tower is not None and any(k.startswith("model.video_tower.video_tower.") for k in sd):
