@@ -180,6 +180,28 @@ int vb200_attention_ws(const void* q, const void* k, const void* v, void* out, i
                        float scale, int causal, const int32_t* kv_len, const uint8_t* mask,
                        int64_t m_sb, int64_t m_sh, int64_t m_sq, void* workspace, size_t workspace_bytes,
                        cudaStream_t stream);
+/* Paged prefill attention (attention_tc.cu): a chunk of new queries over keys that sit in the paged KV cache
+ * (k_pages / v_pages [num_pages, H, page_size, head_dim] bf16, block_table int32 [B, max_pages], as in the decode path
+ * below). q [B, Sq, H, head_dim] with element strides (q_sb, q_ss, q_sh), e.g. the q third of the fused qkv rows after
+ * vb200_rope_kv_append has rotated them and written the chunk's K / V to its pages. Row b holds q_len[b] <= Sq queries
+ * (int32 device arrays q_start / q_len [B]) at cache positions q_start[b] + i: key j is visible to query i iff
+ * j <= q_start[b] + i; keys come from page block_table[b, j / page_size]. Query rows i >= q_len[b] are written as zeros.
+ * q_start[b] + q_len[b] <= max_kv_len <= max_pages * page_size; keys at or past max_kv_len are never attended and
+ * block-table entries past ceil(max_kv_len / page_size) are never read. Pages are loaded whole: the V values of every slot
+ * in a page a row reads must be finite, including slots past its visible keys (they enter P·V with weight 0, and 0 · NaN
+ * is NaN); a zero-initialised cache, as PagedKVCache keeps, satisfies this. block_table rows are max_pages apart.
+ * Stands in for HF LlamaAttention with past_key_values (transformers 4.31: torch.cat of the cache, causal mask offset by
+ * the past length). head_dim 128 and page_size 64 only (else VB_ERR_UNSUPPORTED). Strides multiples of 8, q / out /
+ * pages 16-byte aligned. A grid of fewer (128-query tile, head, row) CTAs than SMs is split over the keys through the
+ * workspace reported by vb200_attention_paged_workspace_size (0 = unsplit; with workspace == NULL the call runs
+ * unsplit); the partials are merged in a fixed order, so repeated calls are bit-identical. */
+size_t vb200_attention_paged_workspace_size(int64_t B, int64_t H, int64_t Sq, int64_t head_dim, int64_t max_kv_len);
+int vb200_attention_paged(const void* q, int64_t q_sb, int64_t q_ss, int64_t q_sh, const void* k_pages,
+                          const void* v_pages, int64_t num_pages, const int32_t* block_table, int64_t max_pages,
+                          const int32_t* q_start, const int32_t* q_len, void* out, int64_t o_sb, int64_t o_ss,
+                          int64_t o_sh, int64_t B, int64_t H, int64_t Sq, int64_t head_dim, int64_t page_size,
+                          int64_t max_kv_len, float scale, void* workspace, size_t workspace_bytes,
+                          cudaStream_t stream);
 /* tiny sequences (S <= 32, head_dim 64): temporal attention of the video tower
  * (modeling_video.py:105-127) and of TemporalTransformer (util.py:1061-1066). */
 int vb200_attention_short(const void* q, const void* k, const void* v, void* out, int64_t nseq,

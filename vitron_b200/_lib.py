@@ -55,6 +55,9 @@ SIGNATURES = {
     "vb200_attention_workspace_size": (_sz, [_i64, _i64, _i64, _i64, _i64, _i32]),
     "vb200_attention_ws": (_i32, [_p, _p, _p, _p, _i64, _i64, _i64, _i64, _i64] + [_i64] * 12 +
                            [_f, _i32, _p, _p, _i64, _i64, _i64, _p, _sz, _p]),
+    "vb200_attention_paged_workspace_size": (_sz, [_i64, _i64, _i64, _i64, _i64]),
+    "vb200_attention_paged": (_i32, [_p, _i64, _i64, _i64, _p, _p, _i64, _p, _i64, _p, _p, _p, _i64, _i64, _i64,
+                                     _i64, _i64, _i64, _i64, _i64, _i64, _f, _p, _sz, _p]),
     "vb200_attention_short": (_i32, [_p, _p, _p, _p, _i64, _i64, _i64, _i64] + [_i64] * 17 + [_f, _p]),
     "vb200_add_rowgroup": (_i32, [_p, _p, _p, _i64, _i64, _i64, _i64, _p]),
     "vb200_rope_kv_append": (_i32, [_p, _i64, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _f, _p]),

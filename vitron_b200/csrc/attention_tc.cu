@@ -22,6 +22,8 @@
 #include "vitron_b200.h"
 #include "wgmma.cuh"
 
+#include <type_traits>
+
 namespace vb {
 
 constexpr int TC_BM = 128;  // query rows per CTA
@@ -41,6 +43,17 @@ struct TcAttnParams {
   int splits;            // > 1: the key blocks are divided over `splits` CTAs per query tile (few-query attention: SEEM's
   float* ws_o;           //      101 queries over 16384 keys would otherwise run on 8 CTAs); each writes its un-normalised
   float* ws_ml;          //      O (fp32) and (m, l) to the workspace, attn_split_merge_kernel combines them
+};
+
+// Paged instantiation (vb200_attention_paged): K / V come from a paged cache [num_pages, H, 64, 128] through the block
+// table, one 64-key block = one (page, head) box. Row b holds q_len[b] queries at cache positions q_start[b] + i;
+// query i sees key j iff j <= q_start[b] + i (causal, kv_len and mask of the base struct are unused).
+struct TcPagedParams : TcAttnParams {
+  const int32_t* block_table;   // [B, max_pages]
+  int max_pages;
+  const int32_t* q_start;       // [B]
+  const int32_t* q_len;         // [B]
+  int max_kv_len;               // keys at positions >= max_kv_len are never read
 };
 
 // Bounded mbarrier wait: a protocol or descriptor bug must never hang the GPU. After 4 s without progress the
@@ -89,10 +102,11 @@ constexpr int tc_smem_bytes() {
   return TC_BM * HD * 2 + 4 * TC_BN * HD * 2 + 128;   // Q + 2-stage K and V rings + barriers
 }
 
-template <int HD>
+template <int HD, typename P>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                     const __grid_constant__ CUtensorMap tmap_v, const TcAttnParams p) {
+                     const __grid_constant__ CUtensorMap tmap_v, const P p) {
+  constexpr bool PAGED = std::is_same<P, TcPagedParams>::value;
   pdl_trigger();
   pdl_wait();   // (the mbarrier set-up below touches no global data, but the kernel's first TMA load follows at once)
   constexpr int KC = HD / 64;                   // 64-element chunks along the head dim
@@ -118,10 +132,19 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const int qb = blockIdx.x / p.splits, sp = blockIdx.x - qb * p.splits, h = blockIdx.y, b = blockIdx.z;
   const int q0 = qb * TC_BM;
-  const int kv_len = p.kv_len ? min(p.kv_len[b], p.Skv) : p.Skv;
-  const int causal_off = p.Skv - p.Sq;
-  int kv_end = kv_len;
-  if (p.causal) kv_end = min(kv_len, q0 + TC_BM + causal_off);
+  int causal_off, kv_end;
+  int q_valid = p.Sq;   // query rows at or past it are written as zeros (paged: q_len[b])
+  if constexpr (PAGED) {
+    const int qs = max(p.q_start[b], 0);
+    q_valid = max(0, min(p.q_len[b], p.Sq));
+    causal_off = qs;
+    kv_end = q0 < q_valid ? min(qs + min(q0 + TC_BM, q_valid), p.max_kv_len) : 0;
+  } else {
+    const int kv_len = p.kv_len ? min(p.kv_len[b], p.Skv) : p.Skv;
+    causal_off = p.Skv - p.Sq;
+    kv_end = kv_len;
+    if (p.causal) kv_end = min(kv_len, q0 + TC_BM + causal_off);
+  }
   const int nblk_all = kv_end > 0 ? (kv_end + TC_BN - 1) / TC_BN : 0;
   // this CTA's share of the key blocks: [jb0, jb0 + nblk)
   const int per_split = (nblk_all + p.splits - 1) / p.splits;
@@ -149,17 +172,40 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
       mbar_arrive_expect_tx(q_full, Q_BYTES);
 #pragma unroll
       for (int c = 0; c < KC; ++c) tma_load_4d(sQ + c * (TC_BM * 128), &tmap_q, q_full, c * 64, q0, h, b);
+      // paged: key block (jb0 + j) is the (page, head) box of the row's (jb0 + j)-th page; the id of the next block's page
+      // is loaded one iteration ahead, so its global-load latency overlaps the wait for a free ring slot
+      const int32_t* pages = nullptr;
+      int next_page = 0;
+      if constexpr (PAGED) {
+        pages = p.block_table + static_cast<long long>(b) * p.max_pages + jb0;
+        next_page = pages[0];
+      }
       for (int j = 0; j < nblk; ++j) {
         const int st = j & 1;
         const uint32_t ph = (j >> 1) & 1;
+        int page = 0;
+        if constexpr (PAGED) {
+          page = next_page;
+          if (j + 1 < nblk) next_page = pages[j + 1];
+        }
         tc_wait(&k_empty[st], ph ^ 1, abort_flag, 5);
         mbar_arrive_expect_tx(&k_full[st], K_BYTES);
+        if constexpr (PAGED) {
 #pragma unroll
-        for (int c = 0; c < KC; ++c) tma_load_4d(sK + st * K_BYTES + c * (TC_BN * 128), &tmap_k, &k_full[st], c * 64, (jb0 + j) * TC_BN, h, b);
+          for (int c = 0; c < KC; ++c) tma_load_4d(sK + st * K_BYTES + c * (TC_BN * 128), &tmap_k, &k_full[st], c * 64, 0, h, page);
+        } else {
+#pragma unroll
+          for (int c = 0; c < KC; ++c) tma_load_4d(sK + st * K_BYTES + c * (TC_BN * 128), &tmap_k, &k_full[st], c * 64, (jb0 + j) * TC_BN, h, b);
+        }
         tc_wait(&v_empty[st], ph ^ 1, abort_flag, 6);
         mbar_arrive_expect_tx(&v_full[st], V_BYTES);
+        if constexpr (PAGED) {
 #pragma unroll
-        for (int c = 0; c < KC; ++c) tma_load_4d(sV + st * V_BYTES + c * (TC_BN * 128), &tmap_v, &v_full[st], c * 64, (jb0 + j) * TC_BN, h, b);
+          for (int c = 0; c < KC; ++c) tma_load_4d(sV + st * V_BYTES + c * (TC_BN * 128), &tmap_v, &v_full[st], c * 64, 0, h, page);
+        } else {
+#pragma unroll
+          for (int c = 0; c < KC; ++c) tma_load_4d(sV + st * V_BYTES + c * (TC_BN * 128), &tmap_v, &v_full[st], c * 64, (jb0 + j) * TC_BN, h, b);
+        }
       }
     }
     return;
@@ -178,7 +224,7 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   float m_run[2] = {-INFINITY, -INFINITY};   // running row max (score units)
   float l_part[2] = {0.f, 0.f};              // this thread's share of the row sums (quad-reduced at the end)
   const uint8_t* mrow[2] = {nullptr, nullptr};
-  if (p.mask != nullptr) {
+  if (!PAGED && p.mask != nullptr) {
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int qrow = q0 + r_lo + 8 * hh;
@@ -281,6 +327,12 @@ flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const int qrow = q0 + r_lo + 8 * hh;
     if (qrow >= p.Sq) continue;
+    if (PAGED && qrow >= q_valid) {   // padding query of a shorter row: zeros (split: an empty partial)
+      l = 0.f;
+      m_run[hh] = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < HD / 8; ++i) o[4 * i + 2 * hh] = o[4 * i + 2 * hh + 1] = 0.f;
+    }
     if (p.splits > 1) {
       const long long slot = ((static_cast<long long>(b) * p.H + h) * p.splits + sp) * p.Sq + qrow;
       if ((lane & 3) == 0) {
@@ -366,12 +418,12 @@ static int make_qkv_map(CUtensorMap* m, const void* base, long long B, long long
   return r == CUDA_SUCCESS ? VB_OK : VB_ERR_DRIVER;
 }
 
-template <int HD>
-static int launch_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcAttnParams& p,
+template <int HD, typename P>
+static int launch_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const P& p,
                      cudaStream_t stream) {
   constexpr int smem = tc_smem_bytes<HD>();
   static bool attr = false;
-  auto kern = flash_attn_tc_kernel<HD>;
+  auto kern = flash_attn_tc_kernel<HD, P>;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
@@ -414,12 +466,12 @@ extern "C" int vb200_attention_tc_occupancy(int head_dim) {
   cudaError_t e;
   if (head_dim == 64) {
     constexpr int smem = tc_smem_bytes<64>();
-    cudaFuncSetAttribute(flash_attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, flash_attn_tc_kernel<64>, TC_THREADS, smem);
+    cudaFuncSetAttribute(flash_attn_tc_kernel<64, TcAttnParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, flash_attn_tc_kernel<64, TcAttnParams>, TC_THREADS, smem);
   } else if (head_dim == 128) {
     constexpr int smem = tc_smem_bytes<128>();
-    cudaFuncSetAttribute(flash_attn_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, flash_attn_tc_kernel<128>, TC_THREADS, smem);
+    cudaFuncSetAttribute(flash_attn_tc_kernel<128, TcAttnParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, flash_attn_tc_kernel<128, TcAttnParams>, TC_THREADS, smem);
   } else {
     return VB_ERR_ARG;
   }
@@ -496,4 +548,80 @@ int vb_attention_tc(const void* q, const void* k, const void* v, void* out, int6
   if (head_dim <= 64) return launch_tc<64>(tq, tk, tv, p, stream);
   if (head_dim <= 128) return launch_tc<128>(tq, tk, tv, p, stream);
   return launch_tc<192>(tq, tk, tv, p, stream);
+}
+
+// ---------------------------------------------------------------- paged prefill: a chunk of queries over the KV cache
+// split-KV factor of the paged kernel: a chunk whose (query tile, head, batch) grid fills at most half the SMs (a one-user
+// chat turn: 32 CTAs) has its key blocks divided so that the split grid still fits one wave of 2 CTAs per SM, at least
+// 2 key blocks per split (a grid closer to one CTA per SM runs faster unsplit: the split one would need a second wave)
+static int paged_splits(int64_t B, int64_t H, int64_t Sq, int64_t max_kv_len) {
+  const long long ctas = ((Sq + TC_BM - 1) / TC_BM) * H * B;
+  const long long nblk = (max_kv_len + TC_BN - 1) / TC_BN;
+  const int sms = vb_num_sms();
+  if (ctas * 2 > sms || nblk < 4) return 1;
+  long long s = 2LL * sms / ctas;
+  if (s > nblk / 2) s = nblk / 2;
+  if (s > 32) s = 32;
+  return s < 2 ? 1 : static_cast<int>(s);
+}
+
+extern "C" size_t vb200_attention_paged_workspace_size(int64_t B, int64_t H, int64_t Sq, int64_t head_dim,
+                                                       int64_t max_kv_len) {
+  if (B <= 0 || H <= 0 || Sq <= 0 || head_dim != 128 || max_kv_len <= 0) return 0;
+  const int s = paged_splits(B, H, Sq, max_kv_len);
+  if (s <= 1) return 0;
+  return static_cast<size_t>(s) * B * H * Sq * (128 + 2) * sizeof(float);
+}
+
+extern "C" int vb200_attention_paged(const void* q, int64_t q_sb, int64_t q_ss, int64_t q_sh, const void* k_pages,
+                                     const void* v_pages, int64_t num_pages, const int32_t* block_table, int64_t max_pages,
+                                     const int32_t* q_start, const int32_t* q_len, void* out, int64_t o_sb, int64_t o_ss,
+                                     int64_t o_sh, int64_t B, int64_t H, int64_t Sq, int64_t head_dim, int64_t page_size,
+                                     int64_t max_kv_len, float scale, void* workspace, size_t workspace_bytes,
+                                     cudaStream_t stream) {
+  VB_CHECK_ARG(q && k_pages && v_pages && block_table && q_start && q_len && out);
+  VB_CHECK_ARG(B > 0 && H > 0 && Sq > 0 && head_dim > 0 && page_size > 0 && num_pages > 0 && max_pages > 0);
+  VB_CHECK_ARG(B <= 65535 && H <= 65535 && Sq <= (1LL << 30) && num_pages <= (1LL << 31) - 1 && max_pages <= (1LL << 24));
+  VB_CHECK_ARG(max_kv_len > 0 && max_kv_len <= max_pages * page_size);
+  const int64_t st[6] = {q_sb, q_ss, q_sh, o_sb, o_ss, o_sh};
+  for (int i = 0; i < 6; ++i) VB_CHECK_ARG(st[i] >= 0 && st[i] % 8 == 0);
+  VB_CHECK_ARG(q_ss > 0 && o_ss > 0);
+  VB_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(k_pages) |
+                 reinterpret_cast<uintptr_t>(v_pages)) & 15) == 0);
+  if (head_dim != 128 || page_size != TC_BN) return VB_ERR_UNSUPPORTED;
+  // a tensor-map dim of extent > 1 needs a non-zero stride (as in vb_attention_tc)
+  VB_CHECK_ARG((B == 1 || q_sb > 0) && (H == 1 || q_sh > 0));
+  auto fix = [](int64_t stride, int64_t fallback) { return stride == 0 ? fallback : stride; };
+  const int64_t page_elems = TC_BN * head_dim;
+  CUtensorMap tq, tk, tv;
+  if (int r = make_qkv_map(&tq, q, B, Sq, H, head_dim, fix(q_sb, q_ss * Sq), q_ss, fix(q_sh, q_ss * Sq), TC_BM)) return r;
+  // the cache as [num_pages, 64 keys, H, D] views: coordinate (d, key, head, page)
+  if (int r = make_qkv_map(&tk, k_pages, num_pages, TC_BN, H, head_dim, H * page_elems, head_dim, page_elems, TC_BN)) return r;
+  if (int r = make_qkv_map(&tv, v_pages, num_pages, TC_BN, H, head_dim, H * page_elems, head_dim, page_elems, TC_BN)) return r;
+  TcPagedParams p;
+  p.o = reinterpret_cast<bf16*>(out);
+  p.o_sb = o_sb; p.o_ss = o_ss; p.o_sh = o_sh;
+  p.B = static_cast<int>(B); p.H = static_cast<int>(H); p.Sq = static_cast<int>(Sq);
+  p.Skv = static_cast<int>(max_kv_len);
+  p.D = static_cast<int>(head_dim);
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.causal = 1;
+  p.kv_len = nullptr;
+  p.mask = nullptr;
+  p.m_sb = p.m_sh = p.m_sq = 0;
+  p.block_table = block_table;
+  p.max_pages = static_cast<int>(max_pages);
+  p.q_start = q_start;
+  p.q_len = q_len;
+  p.max_kv_len = static_cast<int>(max_kv_len);
+  p.splits = 1;
+  p.ws_o = nullptr;
+  p.ws_ml = nullptr;
+  const size_t need = vb200_attention_paged_workspace_size(B, H, Sq, head_dim, max_kv_len);
+  if (need > 0 && workspace != nullptr && workspace_bytes >= need && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0) {
+    p.splits = paged_splits(B, H, Sq, max_kv_len);
+    p.ws_o = reinterpret_cast<float*>(workspace);
+    p.ws_ml = p.ws_o + static_cast<size_t>(p.splits) * B * H * Sq * 128;
+  }
+  return launch_tc<128>(tq, tk, tv, p, stream);
 }

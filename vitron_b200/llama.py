@@ -294,10 +294,11 @@ class LlamaEngine:
         return n
 
     # ------------------------------------------------------------------ layers
-    def _layer(self, i, h, positions, bot, slots, prefill_shape=None, kv_len=None, max_kv_len=0):
+    def _layer(self, i, h, positions, bot, slots, prefill_shape=None, kv_len=None, max_kv_len=0, q_start=None):
         """h [T, d] is updated in place and returned. RMSNorm is never a kernel of its own: its gain is
         folded into wqkv / wgu and 1/rms is a row scale of the GEMM epilogue (computed inside the
-        weight-streaming kernel for T <= 16)."""
+        weight-streaming kernel for T <= 16). With q_start (append) the chunk attends over the paged cache: kv_len is
+        then the chunk length per row and max_kv_len the longest cached + chunk length."""
         c, L, cache = self.cfg, self.layers[i], self.cache
         H, D = c.num_attention_heads, c.head_dim
         g1, g2 = L.get("g1"), L.get("g2")        # RMSNorm gains of NF4 layers (bf16 layers have them folded in)
@@ -307,7 +308,11 @@ class LlamaEngine:
             ops.rope_kv_append(qkv, positions, H, D, c.rope_theta, cache.k(i), cache.v(i), cache.block_table, bot, slots,
                                cache.page_size)
             q4 = qkv.view(B, S, 3, H, D)
-            att = ops.attention(q4[:, :, 0], q4[:, :, 1], q4[:, :, 2], causal=True, kv_len=kv_len)
+            if q_start is None:
+                att = ops.attention(q4[:, :, 0], q4[:, :, 1], q4[:, :, 2], causal=True, kv_len=kv_len)
+            else:   # the chunk's K / V were just scattered to their pages: every key is read from the cache
+                att = ops.attention_paged(q4[:, :, 0], cache.k(i), cache.v(i), cache.block_table[:B], q_start, kv_len,
+                                          max_kv_len)
             att = att.view(B * S, H * D)
         else:  # decode: RoPE + KV append happen inside the attention kernel
             att = ops.attn_decode_rope(qkv, self._rope_tab, cache.k(i), cache.v(i), cache.block_table, kv_len, H, D,
@@ -359,6 +364,52 @@ class LlamaEngine:
         last = (torch.arange(B) * S + (lens_t.long() - 1)).to(dev)
         hl = h.index_select(0, last)
         return ops.gemm(hl, self.lm_head, out_fp32=True, rms_eps=c.rms_norm_eps)
+
+    # ------------------------------------------------------------------ append
+    def append(self, inputs_embeds, chunk_lens, all_logits=True, past_lens=None):
+        """Extend the cached sequences of slots 0..B-1 by a chunk: inputs_embeds [B, S, d] bf16 (right padded),
+        chunk_lens = valid tokens per row. past_lens (default: the lengths the last prefill / append left) = cached
+        tokens each row continues from; positions at or past it are overwritten, so appending twice from the same past
+        branches. Returns fp32 logits of every chunk position [B, S, V] (or of the last valid one [B, V])."""
+        c, dev, cache = self.cfg, self.device, self.cache
+        B, S, d = inputs_embeds.shape
+        if B > self.max_batch:
+            raise ValueError(f"batch {B} > engine max_batch {self.max_batch}")
+        past = list(self._lens_host[:B]) if past_lens is None else [int(x) for x in past_lens]
+        lens = [int(x) for x in chunk_lens]
+        if len(past) != B or len(lens) != B or min(lens) < 1 or max(lens) > S or min(past) < 0:
+            raise ValueError(f"chunk lengths {lens} / past lengths {past} do not fit a [{B}, {S}] chunk")
+        total = [p + n for p, n in zip(past, lens)]
+        if max(total) > cache.max_seq_len:
+            raise ValueError(f"prompt of {max(total)} tokens exceeds the KV cache capacity {cache.max_seq_len} "
+                             f"(construct the model with a larger max_seq_len)")
+        changed = False
+        for b in range(B):
+            changed |= cache.reserve(b, total[b])
+        if changed:
+            cache.sync_table()
+        ar = torch.arange(S, dtype=torch.int32)
+        past_t, lens_t = torch.tensor(past, dtype=torch.int32), torch.tensor(lens, dtype=torch.int32)
+        pos_h = (past_t[:, None] + ar[None, :]).reshape(-1)
+        valid = (ar[None, :] < lens_t[:, None]).reshape(-1)
+        slots_h = torch.where(valid, pos_h, torch.full_like(pos_h, -1))      # -1: padding, the K/V scatter skips it
+        bot_h = torch.arange(B, dtype=torch.int32).repeat_interleave(S)
+        positions, slots, bot = (t.to(dev, non_blocking=True) for t in (pos_h, slots_h, bot_h))
+        q_start, q_len = past_t.to(dev, non_blocking=True), lens_t.to(dev, non_blocking=True)
+        h = inputs_embeds.to(BF16).reshape(B * S, d).clone()
+        for i in range(c.num_hidden_layers):
+            self._layer(i, h, positions, bot, slots, prefill_shape=(B, S), kv_len=q_len, max_kv_len=max(total),
+                        q_start=q_start)
+        # decode state continues after the chunk, as after a prefill of the whole sequence
+        tot_t = torch.tensor(total, dtype=torch.int32).to(dev, non_blocking=True)
+        self.d_pos[:B].copy_(tot_t)
+        self.d_len[:B].copy_(tot_t + 1)
+        self.d_prompt[:B].copy_(tot_t)
+        self._lens_host = list(total)
+        if all_logits:
+            return ops.gemm(h, self.lm_head, out_fp32=True, rms_eps=c.rms_norm_eps).view(B, S, c.vocab_size)
+        last = (torch.arange(B) * S + (lens_t.long() - 1)).to(dev)
+        return ops.gemm(h.index_select(0, last), self.lm_head, out_fp32=True, rms_eps=c.rms_norm_eps)
 
     # ------------------------------------------------------------------ decode
     def _decode_body(self, B):

@@ -372,6 +372,29 @@ def attention(q, k, v, scale=None, causal=False, kv_len=None, mask=None, out=Non
     return out
 
 
+def attention_paged(q, k_pages, v_pages, block_table, q_start, q_len, max_kv_len, scale=None, out=None):
+    """A chunk of queries over the paged KV cache (vb200_attention_paged): q [B, Sq, H, 128] strided view with RoPE
+    applied, k_pages / v_pages [num_pages, H, 64, 128], block_table int32 [B, max_pages] (contiguous), q_start /
+    q_len int32 [B] on the device (keys cached before the chunk, valid queries), max_kv_len >= q_start + q_len on the host.
+    -> [B, Sq, H, 128]; query i of row b sees keys j <= q_start[b] + i, rows i >= q_len[b] are zeros."""
+    lib = _lib.load()
+    B, Sq, H, D = q.shape
+    scale = 1.0 / math.sqrt(D) if scale is None else scale
+    _req(block_table.dim() == 2 and block_table.shape[0] >= B and block_table.is_contiguous(),
+         "block_table: contiguous int32 [>= B, max_pages]")
+    _req(k_pages.is_contiguous() and v_pages.is_contiguous() and k_pages.shape == v_pages.shape, "contiguous pages")
+    if out is None:
+        out = torch.empty((B, Sq, H, D), dtype=BF16, device=q.device)
+    need = lib.vb200_attention_paged_workspace_size(B, H, Sq, D, int(max_kv_len))
+    ws = workspace(need, q.device, "attn") if need else None
+    check(lib.vb200_attention_paged(q.data_ptr(), *_bsh(q), k_pages.data_ptr(), v_pages.data_ptr(), k_pages.shape[0],
+                                    block_table.data_ptr(), block_table.shape[1], q_start.data_ptr(), q_len.data_ptr(),
+                                    out.data_ptr(), *_bsh(out), B, H, Sq, D, k_pages.shape[2], int(max_kv_len),
+                                    float(scale), _ptr(ws), need, _stream()), "vb200_attention_paged")
+    _launches[0] += 2 if need else 1
+    return out
+
+
 def set_attention_impl(impl):
     """0 = automatic, 1 = mma.sync kernel only, 2 = wgmma kernel whenever the shape is supported."""
     check(_lib.load().vb200_set_attention_impl(int(impl)), "vb200_set_attention_impl")

@@ -147,6 +147,43 @@ class CausalLMOutput(SimpleNamespace):
     pass
 
 
+class PagedPast:
+    """`past_key_values` of VitronLlamaForCausalLM.forward: a handle on the rows of the engine's paged KV cache, not a
+    copy. `lens[b]` = tokens cached for row b (image features counted as the positions they fill), `seq_len` = the
+    longest. `len(past)` is the layer count and `past[layer]` gathers that layer's (k, v) as [B, H, seq_len, head_dim]
+    copies (row b's keys at [0, lens[b]), zeros after), so reference code such as `past[-1][-1].shape[-2]` works.
+
+    A handle stays usable while the cache positions it covers are intact: appending from it (even twice: branching)
+    keeps it valid; generate(), a forward without past_key_values, or an append from a shorter handle that overwrote
+    positions below its length make it stale, and using a stale handle raises ValueError."""
+
+    def __init__(self, model, lens, segments):
+        self._model, self.lens, self._segments = model, list(lens), segments
+
+    @property
+    def seq_len(self):
+        return max(self.lens)
+
+    def __len__(self):
+        return self._model.engine.cfg.num_hidden_layers
+
+    def __getitem__(self, layer):
+        self._model._check_past(self)
+        eng = self._model.engine
+        cache, c = eng.cache, eng.cfg
+        i = range(c.num_hidden_layers)[layer]
+        B, S = len(self.lens), self.seq_len
+        out = []
+        for pages in (cache.k(i), cache.v(i)):
+            t = torch.zeros((B, c.num_attention_heads, S, c.head_dim), dtype=pages.dtype, device=pages.device)
+            for b, n in enumerate(self.lens):
+                idx = torch.tensor(cache._owned[b][:(n + cache.page_size - 1) // cache.page_size], dtype=torch.long,
+                                   device=pages.device)
+                t[b, :, :n] = pages[idx].permute(1, 0, 2, 3).reshape(c.num_attention_heads, -1, c.head_dim)[:, :n]
+            out.append(t)
+        return tuple(out)
+
+
 class VitronLlamaForCausalLM(ModuleFace):
     def __init__(self, config, device="cuda", max_batch=8, max_seq_len=2048):
         self.config = config
@@ -337,11 +374,14 @@ class VitronLlamaForCausalLM(ModuleFace):
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, past_key_values=None,
                 inputs_embeds=None, labels=None, use_cache=None, output_attentions=None,
                 output_hidden_states=None, images=None, regions=None, return_dict=None):
-        """Full-sequence forward: logits for every position (fp32), like the reference with
-        past_key_values=None. (Incremental decoding goes through `generate`, which keeps the KV cache
-        inside the engine.)"""
+        """Logits for every position (fp32), like the reference. use_cache=True returns a PagedPast handle as
+        `past_key_values`; passing it back appends the chunk (input_ids [B, n], attention_mask [B, past + n] that is 1
+        over the chunk and whose past part sums to the handle's row lengths) to the cached rows and returns the chunk's
+        logits [B, n, V] and a handle covering past + n. An image inside the chunk is spliced as in a first forward."""
         if past_key_values is not None:
-            raise NotImplementedError("incremental forward() is internal to generate(); pass past_key_values=None")
+            return self._forward_chunk(input_ids, attention_mask, past_key_values, inputs_embeds, labels, use_cache,
+                                       images, regions)
+        self._kv_segments = None          # the prefill below overwrites the cache: every handle becomes stale
         if inputs_embeds is None:
             if images is not None:
                 (input_ids, position_ids, attention_mask, past_key_values, inputs_embeds, labels) = \
@@ -353,13 +393,76 @@ class VitronLlamaForCausalLM(ModuleFace):
         logits = self.engine.prefill(embeds, lens, all_logits=True)
         if restore is not None:
             logits = restore(logits)
-        loss = None
-        if labels is not None:
-            sl = logits[:, :-1].reshape(-1, logits.shape[-1])
-            loss = torch.nn.functional.cross_entropy(sl, labels[:, 1:].reshape(-1).to(sl.device), ignore_index=IGNORE_INDEX)
-        return CausalLMOutput(loss=loss, logits=logits, past_key_values=None, hidden_states=None, attentions=None)
+        past = self._new_past(lens, None) if use_cache else None
+        return CausalLMOutput(loss=self._loss(logits, labels), logits=logits, past_key_values=past, hidden_states=None,
+                              attentions=None)
 
     __call__ = forward
+
+    @staticmethod
+    def _loss(logits, labels):
+        if labels is None:
+            return None
+        sl = logits[:, :-1].reshape(-1, logits.shape[-1])
+        return torch.nn.functional.cross_entropy(sl, labels[:, 1:].reshape(-1).to(sl.device), ignore_index=IGNORE_INDEX)
+
+    # ------------------------------------------------------------------ KV-cache handles
+    # self._kv_segments[b] lists (end, write id) of the writes that produced cache positions [0, end) of row b; a handle
+    # records the list its positions came from and is valid while that list is still a prefix of the current one.
+    _kv_segments = None
+    _kv_writes = 0
+
+    def _new_past(self, lens, parent):
+        self._kv_writes += 1
+        w = self._kv_writes
+        base = parent._segments if parent is not None else [[] for _ in lens]
+        segs = [list(s) + [(n, w)] for s, n in zip(base, lens)]
+        self._kv_segments = segs
+        return PagedPast(self, lens, segs)
+
+    def _check_past(self, past):
+        if not isinstance(past, PagedPast):
+            raise ValueError("past_key_values must be the PagedPast handle a forward(use_cache=True) of this model returned "
+                             "(tuples of cache tensors are not accepted)")
+        cur = self._kv_segments
+        if (past._model is not self or cur is None or len(cur) != len(past._segments)
+                or any(c[:len(s)] != s for c, s in zip(cur, past._segments))):
+            raise ValueError("stale past_key_values: the KV cache positions it covers were overwritten since (generate(), "
+                             "a forward without past_key_values, or an append from a shorter handle)")
+
+    def _forward_chunk(self, input_ids, attention_mask, past, inputs_embeds, labels, use_cache, images, regions):
+        self._check_past(past)
+        B = len(past.lens)
+        n = (input_ids if inputs_embeds is None else inputs_embeds).shape[1]
+        if (input_ids if inputs_embeds is None else inputs_embeds).shape[0] != B:
+            raise ValueError(f"chunk of {(input_ids if inputs_embeds is None else inputs_embeds).shape[0]} rows for a "
+                             f"past of {B} rows")
+        if attention_mask is not None:
+            am = attention_mask.detach().cpu().bool()
+            if am.shape[0] != B or am.shape[1] < n or not bool(am[:, am.shape[1] - n:].all()):
+                raise ValueError(f"attention_mask must be [B, past + {n}] with ones over the chunk")
+            if am[:, :am.shape[1] - n].sum(1).tolist() != past.lens:
+                raise ValueError(f"the past part of attention_mask covers {am[:, :am.shape[1] - n].sum(1).tolist()} "
+                                 f"tokens per row, the handle caches {past.lens}")
+        chunk_mask = torch.ones((B, n), dtype=torch.long, device=(input_ids if inputs_embeds is None else inputs_embeds).device)
+        am_chunk = None
+        if inputs_embeds is None:
+            if images is not None and n > 1:
+                _, _, am_chunk, _, inputs_embeds, labels = self.prepare_inputs_labels_for_multimodal(
+                    input_ids, None, chunk_mask, past, labels, images, regions)
+            else:
+                inputs_embeds = self.model.embed_tokens(input_ids)
+        embeds, lens, restore = self._right_pad(inputs_embeds, am_chunk)
+        logits = self.engine.append(embeds, lens, all_logits=True, past_lens=past.lens)
+        if restore is not None:
+            logits = restore(logits)
+        total = [p + m for p, m in zip(past.lens, lens)]
+        # the chunk's K / V now occupy positions past.lens.. of the cache whatever use_cache is: the write is recorded, so
+        # that a handle whose positions it overwrote is seen as stale
+        new_past = self._new_past(total, past)
+        return CausalLMOutput(loss=self._loss(logits, labels), logits=logits,
+                              past_key_values=new_past if use_cache is not False else None, hidden_states=None,
+                              attentions=None)
 
     def _right_pad(self, embeds, attention_mask):
         """Engine wants right-padded rows. Returns (embeds, lens, restore_fn or None)."""
@@ -403,6 +506,7 @@ class VitronLlamaForCausalLM(ModuleFace):
         pad = self.config.pad_token_id if pad_token_id is None else pad_token_id
         eos_set = set(eos if isinstance(eos, (list, tuple)) else [eos]) if eos is not None else set()
         B = input_ids.shape[0]
+        self._kv_segments = None          # the prefill and decode below overwrite the cache: every handle becomes stale
         if images is not None:
             _, _, am, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(
                 input_ids, None, attention_mask if attention_mask is not None else torch.ones_like(input_ids),
