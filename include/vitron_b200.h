@@ -241,6 +241,15 @@ int vb200_attn_decode_rope(const void* qkv, int64_t ld_qkv, const float* rope_ta
                            const int32_t* kv_len, void* out, int64_t ld_o, int64_t B, int64_t n_heads,
                            int64_t head_dim, int64_t page_size, int64_t max_kv_len, float scale,
                            void* workspace, size_t workspace_bytes, cudaStream_t stream);
+/* beam-indirect decode step (vb200_attn_decode_rope for beam search): row b reads key j >= gen_start[b] from the pages
+ * of row beam_src[b * src_ld + j], through that row's block table; keys below gen_start (the shared prompt) through its
+ * own. Every row still appends its new token's K / V to its own pages. Requires src_ld >= max_kv_len. */
+int vb200_attn_decode_rope_beam(const void* qkv, int64_t ld_qkv, const float* rope_table, void* k_pages,
+                                void* v_pages, const int32_t* block_table, int64_t max_pages, const int32_t* kv_len,
+                                const int32_t* beam_src, int64_t src_ld, const int32_t* gen_start, void* out,
+                                int64_t ld_o, int64_t B, int64_t n_heads, int64_t head_dim, int64_t page_size,
+                                int64_t max_kv_len, float scale, void* workspace, size_t workspace_bytes,
+                                cudaStream_t stream);
 /* inputs_embeds[b, s] = srcmap >= 0 ? embed[srcmap] : feats[-srcmap-1] : the device half of
  * prepare_inputs_labels_for_multimodal (vitron/model/llava_arch.py:478-521); pad rows (srcmap ==
  * INT32_MIN) are zero-filled. */
@@ -281,6 +290,41 @@ typedef struct vb_sample_params {
 int vb200_sample_advance(const float* logits, int64_t ld, int64_t rows, int64_t n, const vb_sample_params* params,
                          int64_t* out_idx, int32_t* next_src, int32_t* positions, int32_t* kv_len,
                          int64_t* token_log, int64_t log_stride, const int32_t* prompt_len, cudaStream_t stream);
+
+/* Beam-search parameters, read by the kernel from DEVICE memory (one captured decode graph serves every setting). */
+typedef struct vb_beam_params {
+  double length_penalty;   /* a double, as the Python float transformers uses */
+  int32_t early_stopping;  /* 0: False, 1: True, 2: "never" (HF 4.31) */
+  int32_t pad_token_id;
+  int32_t input_len;       /* input_ids.shape[1]: a hypothesis of t generated tokens has length input_len + t */
+  int32_t max_length;      /* input_len + max_new_tokens ("never" with length_penalty > 0) */
+  int32_t n_eos;           /* 0..8 */
+  int32_t eos[8];
+} vb_beam_params;          /* 64 bytes: 4 bytes of tail padding */
+
+/* workspace of vb200_beam_advance: [16 KB of arrival counters (B <= 4096) | candidates]; zero-filled ONCE by the caller */
+size_t vb200_beam_workspace_size(int64_t rows);
+/* beam step of HF 4.31 beam_search for B requests x k beams (row r = b * k + j, 1 <= k <= 16, 2 <= n <= 49152, else
+ * VB_ERR_UNSUPPORTED), stated in float64 in vitron_b200/beam.py:
+ *   score[r, i] = log_softmax(logits[r])[i] + beam_score[r] (fp32; NaN counts as -inf);
+ *   the request's top 2k of the flat [k * n] scores, ties to the lower flat index j * n + i;
+ *   walked in rank order: an EOS (any of params->eos) at rank < k becomes a hypothesis (score / L^length_penalty, L =
+ *   input_len + t, t = kv_len - prompt_len), at rank >= k it is skipped; other candidates fill the k next beams;
+ *   per request at most k hypotheses (hyp_score f64 / hyp_len / hyp_seq [B * k] indexed b * k + slot, hyp_count [B],
+ *   generated ids hyp_ids [B * k, hyp_ld]); the lowest score, earliest added among equals, is evicted;
+ *   done[b] follows BeamHypotheses.is_done (early_stopping True / False / "never"); a done request's beams get
+ *   pad_token_id, score 0 and themselves as parent. If fewer than k non-EOS candidates are left, the missing beams
+ *   continue their own row with pad_token_id and score -1e9 (4.31 raises there).
+ * Bookkeeping of child row c: beam_score, parent (parent row), next_src = token, token_log[c, t] = token,
+ * positions++, kv_len++. beam_src [B * k, src_ld]: entry (c, P + j), P = prompt_len, names the row that logged token j
+ * of c's history and holds its K / V: children copy their parent's entries [P, P + t), then entry P + t = c.
+ * Deterministic: the same inputs give bit-identical outputs whatever the order in which the rows' CTAs finish. */
+int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n, const vb_beam_params* params,
+                       float* beam_score, int32_t* parent, int32_t* done, int32_t* beam_src, int64_t src_ld,
+                       double* hyp_score, int32_t* hyp_len, int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids,
+                       int64_t hyp_ld, int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
+                       int64_t log_stride, const int32_t* prompt_len, void* workspace, size_t workspace_bytes,
+                       cudaStream_t stream);
 
 /* ---- vision / diffusion glue (vision.cu) ----------------------------------------------------
  * patchify: NCHW pixels -> [nb*gh*gw, kpad] rows ordered (c, py, px) for the patch-embed GEMM

@@ -113,13 +113,16 @@ __global__ void rope_table_kernel(const int32_t* __restrict__ positions, float* 
   table[b * 2 * half + half + i] = sn;
 }
 
-template <bool ROPE, int MAX_TRIPS>
+// BEAM: key j >= gen_start[b] of row b is read from the pages of row beam_src[b * src_ld + j] (through that row's block
+// table): the beams of a request share their history without copying it. Keys below gen_start use the row's own table.
+template <bool ROPE, int MAX_TRIPS, bool BEAM = false>
 __global__ void __launch_bounds__(DEC_THREADS, 4)   // 4 CTAs per SM: the one-wave split policy counts on 4 x (SM count) slots
 attn_decode_kernel(const bf16* __restrict__ q, long long ld_q, bf16* __restrict__ k_pages,
                    bf16* __restrict__ v_pages, const int32_t* __restrict__ block_table, int max_pages,
                    const int32_t* __restrict__ kv_len, int H, int page_size, float scale, int splits, int per,
                    float* __restrict__ ws_ml, float* __restrict__ ws_o, int* __restrict__ counters,
-                   bf16* __restrict__ out, long long ld_o, const float* __restrict__ rope_table) {
+                   bf16* __restrict__ out, long long ld_o, const float* __restrict__ rope_table,
+                   const int32_t* __restrict__ beam_src, int src_ld, const int32_t* __restrict__ gen_start) {
   // page_size == 64 and per % 64 == 0 (host-checked): a 64-key trip is exactly one page, and the page ids of
   // this split depend only on (split, per), so they are fetched before anything else (the block table is
   // constant during decoding -> safe ahead of the PDL dependency wait).
@@ -155,6 +158,7 @@ attn_decode_kernel(const bf16* __restrict__ q, long long ld_q, bf16* __restrict_
   pdl_trigger();
   const int len = kv_len[b];
   const int c1 = min(len, c0 + per);
+  const int gstart = BEAM ? gen_start[b] : 0;
 
   float qv[16];
   {
@@ -217,7 +221,15 @@ attn_decode_kernel(const bf16* __restrict__ q, long long ld_q, bf16* __restrict_
     for (int u = 0; u < 2; ++u) {
       const int kk = gid + 16 * u + 32 * (hs & 1);  // key inside the page
       const bool has = c0 + 64 * (hs >> 1) + kk < c1;
-      const long long off = pbase + static_cast<long long>(has ? kk : 0) * HD;
+      long long off = pbase + static_cast<long long>(has ? kk : 0) * HD;
+      if (BEAM) {
+        const int key = c0 + 64 * (hs >> 1) + kk;
+        if (has && key >= gstart) {
+          const int src_row = beam_src[static_cast<long long>(b) * src_ld + key];
+          off = static_cast<long long>(block_table[static_cast<long long>(src_row) * max_pages + key / 64]) * page_stride +
+                head_off + static_cast<long long>(kk) * HD;
+        }
+      }
       h.k[u][0] = *reinterpret_cast<const uint4*>(k_pages + off);
       h.k[u][1] = *reinterpret_cast<const uint4*>(k_pages + off + 8);
       h.v[u][0] = *reinterpret_cast<const uint4*>(v_pages + off);
@@ -676,6 +688,246 @@ sample_advance_kernel(const float* __restrict__ logits, long long ld, int n, con
   }
 }
 
+// ------------------------------------------------------------------ beam search step (HF 4.31 beam_search + BeamSearchScorer)
+// One CTA per row r = b * k + j: log-softmax of the row and its top 2k candidates (score desc, then index asc) by repeated
+// block arg-max, where only the thread that owned the last winner rescans its strided slice. The request's top 2k lie in
+// the union of its rows' top 2k: the CTA that arrives last for request b ranks those k * 2k candidates, runs the scorer
+// and does the bookkeeping of all k rows. Candidate order is total (flat index = j * n + token breaks every tie), so the
+// result does not depend on arrival order.
+constexpr int BM_THREADS = 1024;
+constexpr int BM_MAX_K = 16;
+constexpr int BM_MAX_N = 49152;              // 192 KB of staged row
+constexpr int BM_STAGE = 256;                // beam-source columns staged per pass of the history reorder
+constexpr size_t BM_COUNTER_BYTES = 16384;   // B <= 4096 arrival counters, then the candidates
+constexpr int BM_SENTINEL = 0x40000000;      // flat index of a missing candidate (row with fewer than 2k entries)
+
+__device__ __forceinline__ bool bm_better(float sa, int ia, float sb, int ib) {
+  return sa > sb || (sa == sb && ia < ib);
+}
+
+__global__ void __launch_bounds__(BM_THREADS, 1)
+beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k, const vb_beam_params* __restrict__ prm,
+                    float* __restrict__ beam_score, int32_t* __restrict__ parent, int32_t* __restrict__ done,
+                    int32_t* __restrict__ beam_src, int src_ld, double* __restrict__ hyp_score,
+                    int32_t* __restrict__ hyp_len, int32_t* __restrict__ hyp_seq, int32_t* __restrict__ hyp_count,
+                    int64_t* __restrict__ hyp_ids, int hyp_ld, int32_t* __restrict__ next_src,
+                    int32_t* __restrict__ positions, int32_t* __restrict__ kv_len, int64_t* __restrict__ token_log,
+                    int log_stride, const int32_t* __restrict__ prompt_len, float* __restrict__ cand_s,
+                    int32_t* __restrict__ cand_i, int32_t* __restrict__ counters) {
+  extern __shared__ float srow[];
+  __shared__ float s_f[32];
+  __shared__ int s_i[32];
+  __shared__ float s_ws;
+  __shared__ int s_wi, s_last, s_t, s_P;
+  __shared__ float m_s[BM_MAX_K * 2 * BM_MAX_K];
+  __shared__ int m_i[BM_MAX_K * 2 * BM_MAX_K];
+  __shared__ float t_s[2 * BM_MAX_K];
+  __shared__ int t_i[2 * BM_MAX_K];
+  __shared__ int c_par[BM_MAX_K], c_tok[BM_MAX_K], h_src[BM_MAX_K];
+  __shared__ float c_sc[BM_MAX_K];
+  __shared__ int32_t stage[BM_MAX_K][BM_STAGE];
+  const int r = blockIdx.x, b = r / k, j = r % k, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int k2 = 2 * k;
+  pdl_wait();      // logits, scores and the decode state come from the predecessors
+  pdl_trigger();
+
+  // ---- log-softmax statistics of the row (NaN counts as -inf); fixed reduction order
+  const float* row = logits + r * ld;
+  float mx = -INFINITY;
+  for (int i = tid; i < n; i += BM_THREADS) {
+    float v = row[i];
+    if (v != v) v = -INFINITY;
+    srow[i] = v;
+    mx = fmaxf(mx, v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane == 0) s_f[warp] = mx;
+  __syncthreads();
+  mx = s_f[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  __syncthreads();
+  float sum = 0.f;
+  if (mx > -INFINITY)
+    for (int i = tid; i < n; i += BM_THREADS) sum += expf(srow[i] - mx);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  if (lane == 0) s_f[warp] = sum;
+  __syncthreads();
+  sum = s_f[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  __syncthreads();
+  const float logz = logf(sum);
+  const float bsc = beam_score[r];
+  // candidate score = log_softmax + beam score, as torch computes it: (x - max) - log(sum exp(x - max))
+  auto score_of = [&](int i) -> float { return mx == -INFINITY ? -INFINITY : ((srow[i] - mx) - logz) + bsc; };
+
+  // ---- this row's top 2k
+  float ps = INFINITY;
+  int pi = -1;           // the last candidate this thread supplied: the next one must come after it
+  float my_s;
+  int my_i;
+  auto rescan = [&]() {
+    my_s = -INFINITY;
+    my_i = INT_MAX;
+    for (int i = tid; i < n; i += BM_THREADS) {
+      const float sv = score_of(i);
+      if ((sv < ps || (sv == ps && i > pi)) && bm_better(sv, i, my_s, my_i)) { my_s = sv; my_i = i; }
+    }
+  };
+  rescan();
+  for (int q = 0; q < k2; ++q) {
+    float sv = my_s;
+    int iv = my_i;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float os = __shfl_xor_sync(0xffffffffu, sv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, iv, o);
+      if (bm_better(os, oi, sv, iv)) { sv = os; iv = oi; }
+    }
+    if (lane == 0) { s_f[warp] = sv; s_i[warp] = iv; }
+    __syncthreads();
+    if (warp == 0) {
+      sv = s_f[lane];
+      iv = s_i[lane];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float os = __shfl_xor_sync(0xffffffffu, sv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, iv, o);
+        if (bm_better(os, oi, sv, iv)) { sv = os; iv = oi; }
+      }
+      if (lane == 0) { s_ws = sv; s_wi = iv; }
+    }
+    __syncthreads();
+    const float ws = s_ws;
+    const int wi = s_wi;
+    if (tid == 0) {
+      cand_s[r * 2 * BM_MAX_K + q] = ws;
+      cand_i[r * 2 * BM_MAX_K + q] = wi == INT_MAX ? BM_SENTINEL + r * 2 * BM_MAX_K + q : j * n + wi;
+    }
+    if (wi != INT_MAX && wi % BM_THREADS == tid) { ps = ws; pi = wi; rescan(); }
+  }
+
+  // ---- arrival: the last CTA of request b goes on
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    s_last = atomicAdd(&counters[b], 1) == k - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  const int r0 = b * k, nc = k * k2;
+  for (int c = tid; c < nc; c += BM_THREADS) {
+    const int idx = (r0 + c / k2) * 2 * BM_MAX_K + c % k2;
+    m_s[c] = __ldcg(&cand_s[idx]);
+    m_i[c] = __ldcg(&cand_i[idx]);
+  }
+  __syncthreads();
+  if (tid < nc) {   // rank by counting: flat indices are distinct, so the ranks are a permutation
+    int rank = 0;
+    for (int o = 0; o < nc; ++o) rank += bm_better(m_s[o], m_i[o], m_s[tid], m_i[tid]) ? 1 : 0;
+    if (rank < k2) { t_s[rank] = m_s[tid]; t_i[rank] = m_i[tid]; }
+  }
+  __syncthreads();
+
+  // ---- the scorer (BeamSearchScorer.process + BeamHypotheses.add / is_done), serial over 2k candidates
+  if (tid == 0) {
+    const int t = kv_len[r0] - prompt_len[r0];   // tokens generated before this step
+    const int pad = prm->pad_token_id, in_len = prm->input_len, es = prm->early_stopping;
+    const double lp = prm->length_penalty;
+    for (int c = 0; c < k; ++c) h_src[c] = -1;
+    if (done[b]) {
+      for (int c = 0; c < k; ++c) { c_par[c] = r0 + c; c_tok[c] = pad; c_sc[c] = 0.f; }
+    } else {
+      int cnt = hyp_count[b], filled = 0;
+      auto worst = [&]() -> double {
+        double w = 1e9;
+        for (int s = 0; s < cnt; ++s) w = fmin(w, hyp_score[r0 + s]);
+        return w;
+      };
+      for (int q = 0; q < k2 && filled < k; ++q) {
+        const int f = t_i[q];
+        if (f >= BM_SENTINEL) break;
+        const int bj = f / n, tok = f % n;
+        bool eos = false;
+        for (int e = 0; e < prm->n_eos; ++e) eos |= prm->eos[e] == tok;
+        if (eos) {
+          if (q >= k) continue;
+          const int L = in_len + t;
+          const double sc = static_cast<double>(t_s[q]) / pow(static_cast<double>(L), lp);
+          if (cnt < k || sc > worst()) {
+            int slot = cnt;
+            if (cnt < k) {
+              ++cnt;
+            } else {   // evict the lowest score, the earliest added among equals
+              slot = 0;
+              for (int s = 1; s < cnt; ++s)
+                if (hyp_score[r0 + s] < hyp_score[r0 + slot] ||
+                    (hyp_score[r0 + s] == hyp_score[r0 + slot] && hyp_seq[r0 + s] < hyp_seq[r0 + slot]))
+                  slot = s;
+            }
+            hyp_score[r0 + slot] = sc;
+            hyp_len[r0 + slot] = L;
+            hyp_seq[r0 + slot] = t * 2 * BM_MAX_K + q;
+            h_src[slot] = r0 + bj;
+          }
+        } else {
+          c_par[filled] = r0 + bj; c_tok[filled] = tok; c_sc[filled] = t_s[q];
+          ++filled;
+        }
+      }
+      for (; filled < k; ++filled) { c_par[filled] = r0 + filled; c_tok[filled] = pad; c_sc[filled] = -1e9f; }
+      hyp_count[b] = cnt;
+      if (cnt >= k) {
+        bool d = true;
+        if (es != 1) {
+          const double len = (es == 2 && lp > 0.0) ? static_cast<double>(prm->max_length) : static_cast<double>(in_len + t);
+          d = worst() >= static_cast<double>(t_s[0]) / pow(len, lp);
+        }
+        if (d) done[b] = 1;
+      }
+    }
+    s_t = t;
+    s_P = prompt_len[r0];
+  }
+  __syncthreads();
+  const int t = s_t, P = s_P;
+
+  // ---- generated ids of this step's new hypotheses: token j of row p's history was logged by row beam_src[p][P + j]
+  for (int x = tid; x < k * t; x += BM_THREADS) {
+    const int slot = x / t, jj = x % t, p = h_src[slot];
+    if (p < 0 || jj >= hyp_ld || P + jj >= src_ld || jj >= log_stride) continue;
+    const int w = beam_src[static_cast<long long>(p) * src_ld + P + jj];
+    hyp_ids[static_cast<long long>(r0 + slot) * hyp_ld + jj] = token_log[static_cast<long long>(w) * log_stride + jj];
+  }
+  __syncthreads();
+  // ---- children take their parent's history; every parent column is read before any child column is written
+  const int end = min(P + t, src_ld);
+  for (int c0 = P; c0 < end; c0 += BM_STAGE) {
+    const int w = min(BM_STAGE, end - c0);
+    for (int x = tid; x < k * w; x += BM_THREADS)
+      stage[x / w][x % w] = beam_src[static_cast<long long>(c_par[x / w]) * src_ld + c0 + x % w];
+    __syncthreads();
+    for (int x = tid; x < k * w; x += BM_THREADS)
+      beam_src[static_cast<long long>(r0 + x / w) * src_ld + c0 + x % w] = stage[x / w][x % w];
+    __syncthreads();
+  }
+  if (tid < k) {
+    const int rr = r0 + tid;
+    beam_score[rr] = c_sc[tid];
+    parent[rr] = c_par[tid];
+    next_src[rr] = c_tok[tid];
+    if (t >= 0 && t < log_stride) token_log[static_cast<long long>(rr) * log_stride + t] = c_tok[tid];
+    if (P + t < src_ld) beam_src[static_cast<long long>(rr) * src_ld + P + t] = rr;   // the child writes position P + t next
+    positions[rr] += 1;
+    kv_len[rr] += 1;
+  }
+  if (tid == 0) counters[b] = 0;
+}
+
 }  // namespace vb
 
 using namespace vb;
@@ -711,6 +963,45 @@ extern "C" int vb200_sample_advance(const float* logits, int64_t ld, int64_t row
                             static_cast<size_t>(n) * sizeof(float), stream, logits, static_cast<long long>(ld),
                             static_cast<int>(n), params, out_idx, next_src, positions, kv_len, token_log,
                             static_cast<int>(log_stride), prompt_len);
+  if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
+  return VB_OK;
+}
+
+extern "C" size_t vb200_beam_workspace_size(int64_t rows) {
+  return BM_COUNTER_BYTES + static_cast<size_t>(rows > 0 ? rows : 0) * 2 * BM_MAX_K * (sizeof(float) + sizeof(int32_t));
+}
+
+extern "C" int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                  const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
+                                  int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len,
+                                  int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld,
+                                  int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
+                                  int64_t log_stride, const int32_t* prompt_len, void* workspace,
+                                  size_t workspace_bytes, cudaStream_t stream) {
+  VB_CHECK_ARG(logits && params && beam_score && parent && done && beam_src && hyp_score && hyp_len && hyp_seq &&
+               hyp_count && hyp_ids && next_src && positions && kv_len && token_log && prompt_len);
+  VB_CHECK_ARG(B > 0 && k > 0 && n >= 2 && ld >= n && src_ld > 0 && src_ld <= INT_MAX && hyp_ld > 0 &&
+               hyp_ld <= INT_MAX && log_stride > 0 && log_stride <= INT_MAX);
+  if (k > BM_MAX_K || n > BM_MAX_N || B > static_cast<int64_t>(BM_COUNTER_BYTES / sizeof(int32_t)))
+    return VB_ERR_UNSUPPORTED;
+  const int64_t rows = B * k;
+  if (!workspace || workspace_bytes < vb200_beam_workspace_size(rows)) return VB_ERR_WORKSPACE;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(beam_advance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         BM_MAX_N * static_cast<int>(sizeof(float)));
+    if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
+    attr_set = true;
+  }
+  int32_t* counters = reinterpret_cast<int32_t*>(workspace);
+  float* cand_s = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + BM_COUNTER_BYTES);
+  int32_t* cand_i = reinterpret_cast<int32_t*>(cand_s + rows * 2 * BM_MAX_K);
+  cudaError_t e = vb_launch(beam_advance_kernel, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS),
+                            static_cast<size_t>(n) * sizeof(float), stream, logits, static_cast<long long>(ld),
+                            static_cast<int>(n), static_cast<int>(k), params, beam_score, parent, done, beam_src,
+                            static_cast<int>(src_ld), hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
+                            static_cast<int>(hyp_ld), next_src, positions, kv_len, token_log,
+                            static_cast<int>(log_stride), prompt_len, cand_s, cand_i, counters);
   if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
   return VB_OK;
 }
@@ -778,7 +1069,8 @@ static int launch_attn_decode(const void* q, int64_t ld_q, void* k_pages, void* 
                               const int32_t* block_table, int64_t max_pages, const int32_t* kv_len, void* out,
                               int64_t ld_o, int64_t B, int64_t n_heads, int64_t head_dim, int64_t page_size,
                               int64_t max_kv_len, float scale, void* workspace, size_t workspace_bytes,
-                              const float* rope_table, cudaStream_t stream) {
+                              const float* rope_table, cudaStream_t stream, const int32_t* beam_src = nullptr,
+                              int64_t src_ld = 0, const int32_t* gen_start = nullptr) {
   VB_CHECK_ARG(q && k_pages && v_pages && block_table && kv_len && out);
   VB_CHECK_ARG(B > 0 && n_heads > 0 && page_size > 0 && max_pages > 0);
   if (head_dim != 128) return VB_ERR_UNSUPPORTED;
@@ -801,14 +1093,18 @@ static int launch_attn_decode(const void* q, int64_t ld_q, void* k_pages, void* 
   }
   dim3 grid(splits, static_cast<unsigned>(n_heads), static_cast<unsigned>(B));
   cudaError_t e;
-#define VB_LAUNCH_DECODE(ROPE_, TRIPS_, TABLE_)                                                                    \
-  e = vb_launch(attn_decode_kernel<ROPE_, TRIPS_>, grid, dim3(DEC_THREADS), 0, stream,                            \
+#define VB_LAUNCH_DECODE(ROPE_, TRIPS_, TABLE_, ...)                                                               \
+  e = vb_launch(attn_decode_kernel<ROPE_, TRIPS_, ##__VA_ARGS__>, grid, dim3(DEC_THREADS), 0, stream,             \
                 reinterpret_cast<const bf16*>(q), static_cast<long long>(ld_q), reinterpret_cast<bf16*>(k_pages), \
                 reinterpret_cast<bf16*>(v_pages), block_table, static_cast<int>(max_pages), kv_len,                \
                 static_cast<int>(n_heads), static_cast<int>(page_size), scale, splits, per, ws_ml, ws_o, counters, \
-                reinterpret_cast<bf16*>(out), static_cast<long long>(ld_o), TABLE_)
+                reinterpret_cast<bf16*>(out), static_cast<long long>(ld_o), TABLE_, beam_src,                      \
+                static_cast<int>(src_ld), gen_start)
   const float* no_table = nullptr;
-  if (rope_table != nullptr) {
+  if (beam_src != nullptr) {
+    if (per <= DEC_CHUNK / 2) VB_LAUNCH_DECODE(true, DEC_CHUNK / 128, rope_table, true);
+    else VB_LAUNCH_DECODE(true, DEC_CHUNK / 64, rope_table, true);
+  } else if (rope_table != nullptr) {
     if (per <= DEC_CHUNK / 2) VB_LAUNCH_DECODE(true, DEC_CHUNK / 128, rope_table);
     else VB_LAUNCH_DECODE(true, DEC_CHUNK / 64, rope_table);
   } else {
@@ -850,6 +1146,19 @@ extern "C" int vb200_attn_decode_rope(const void* qkv, int64_t ld_qkv, const flo
   VB_CHECK_ARG(rope_table != nullptr && ld_qkv >= 3 * n_heads * head_dim);
   return launch_attn_decode(qkv, ld_qkv, k_pages, v_pages, block_table, max_pages, kv_len, out, ld_o, B, n_heads,
                             head_dim, page_size, max_kv_len, scale, workspace, workspace_bytes, rope_table, stream);
+}
+
+extern "C" int vb200_attn_decode_rope_beam(const void* qkv, int64_t ld_qkv, const float* rope_table, void* k_pages,
+                                           void* v_pages, const int32_t* block_table, int64_t max_pages,
+                                           const int32_t* kv_len, const int32_t* beam_src, int64_t src_ld,
+                                           const int32_t* gen_start, void* out, int64_t ld_o, int64_t B,
+                                           int64_t n_heads, int64_t head_dim, int64_t page_size, int64_t max_kv_len,
+                                           float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  VB_CHECK_ARG(rope_table != nullptr && ld_qkv >= 3 * n_heads * head_dim);
+  VB_CHECK_ARG(beam_src != nullptr && gen_start != nullptr && src_ld >= max_kv_len && src_ld <= INT_MAX);
+  return launch_attn_decode(qkv, ld_qkv, k_pages, v_pages, block_table, max_pages, kv_len, out, ld_o, B, n_heads,
+                            head_dim, page_size, max_kv_len, scale, workspace, workspace_bytes, rope_table, stream,
+                            beam_src, src_ld, gen_start);
 }
 
 extern "C" int vb200_splice_multimodal(const void* embed, int64_t vocab, const void* feats,

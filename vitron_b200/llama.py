@@ -17,6 +17,7 @@ from dataclasses import dataclass
 import torch
 
 from . import nf4 as _nf4
+from . import beam as _beam
 from . import ops, sampling
 
 BF16 = torch.bfloat16
@@ -55,7 +56,9 @@ class LlamaConfig:
 class PagedKVCache:
     """[layers, 2, num_pages, heads, page_size, head_dim] bf16 + a per-slot block table.
 
-    Pages are handed out from a free list; a sequence slot owns ceil(len / page_size) pages."""
+    Pages are handed out from a free list; a sequence slot owns ceil(len / page_size) pages. fork() lets slots share the
+    full pages of a prompt: every page carries a reference count and returns to the free list when the last slot holding
+    it releases it."""
 
     def __init__(self, cfg, max_batch, max_seq_len, device, page_size=64):
         self.page_size = page_size
@@ -68,6 +71,7 @@ class PagedKVCache:
         self.block_table = torch.zeros((max_batch, self.max_pages), dtype=torch.int32, device=device)
         self._free = list(range(self.num_pages - 1, -1, -1))
         self._owned = [[] for _ in range(max_batch)]
+        self._refs = [0] * self.num_pages
         self.device = device
 
     def reserve(self, slot, length):
@@ -80,12 +84,49 @@ class PagedKVCache:
             if not self._free:
                 raise RuntimeError("KV cache out of pages")
             owned.append(self._free.pop())
+            self._refs[owned[-1]] = 1
             changed = True
         return changed
 
     def release(self, slot):
-        self._free.extend(reversed(self._owned[slot]))
+        for p in reversed(self._owned[slot]):
+            self._refs[p] -= 1
+            if self._refs[p] == 0:
+                self._free.append(p)
         self._owned[slot] = []
+
+    def fork(self, lens, k):
+        """Slots 0..len(lens)-1 hold prompts of lens[b] tokens. Afterwards slot b * k + j (j < k) holds prompt b: its
+        full pages are shared, and the partial last page is copied per slot (its valid tokens, every layer), because
+        the beams write their first generated tokens into it. Call sync_table() afterwards."""
+        B, ps = len(lens), self.page_size
+        src = [self._owned[b][:(lens[b] + ps - 1) // ps] for b in range(B)]
+        for b in range(B):
+            for p in src[b]:
+                self._refs[p] += 1                 # held by the fork until the copies are made
+        for slot in range(max(B, B * k)):
+            self.release(slot)
+        copies = []
+        for b in range(B):
+            full, part = lens[b] // ps, lens[b] % ps
+            for j in range(k):
+                owned = list(src[b][:full])
+                for p in owned:
+                    self._refs[p] += 1
+                if part:
+                    if not self._free:
+                        raise RuntimeError("KV cache out of pages")
+                    owned.append(self._free.pop())
+                    self._refs[owned[-1]] = 1
+                    copies.append((src[b][full], owned[-1], part))
+                self._owned[b * k + j] = owned
+        for old, new, n in copies:
+            self.pages[:, :, new, :, :n] = self.pages[:, :, old, :, :n]
+        for b in range(B):
+            for p in src[b]:
+                self._refs[p] -= 1
+                if self._refs[p] == 0:
+                    self._free.append(p)
 
     def sync_table(self):
         host = torch.zeros((self.max_batch, self.max_pages), dtype=torch.int32)
@@ -127,6 +168,8 @@ class LlamaEngine:
         self.token_log = torch.zeros((B, self.cache.max_seq_len), dtype=torch.int64, device=dev)
         # vb_sample_params read by the sampled step: one captured graph serves every temperature / top-k / top-p / seed
         self.d_sample = torch.zeros((ops.SAMPLE_PARAMS.size,), dtype=torch.uint8, device=dev)
+        self.beam = None       # beam-search state (start_beam), allocated on first use
+        self.beam_k = 0        # beams per request of the current beam search; 0 = no beam search started
         self._graphs = {}
         self.launches_per_step = 0
         self.use_pdl = True
@@ -294,7 +337,8 @@ class LlamaEngine:
         return n
 
     # ------------------------------------------------------------------ layers
-    def _layer(self, i, h, positions, bot, slots, prefill_shape=None, kv_len=None, max_kv_len=0, q_start=None):
+    def _layer(self, i, h, positions, bot, slots, prefill_shape=None, kv_len=None, max_kv_len=0, q_start=None,
+               beam=False):
         """h [T, d] is updated in place and returned. RMSNorm is never a kernel of its own: its gain is
         folded into wqkv / wgu and 1/rms is a row scale of the GEMM epilogue (computed inside the
         weight-streaming kernel for T <= 16). With q_start (append) the chunk attends over the paged cache: kv_len is
@@ -314,6 +358,11 @@ class LlamaEngine:
                 att = ops.attention_paged(q4[:, :, 0], cache.k(i), cache.v(i), cache.block_table[:B], q_start, kv_len,
                                           max_kv_len)
             att = att.view(B * S, H * D)
+        elif beam:   # beam rows read their generated keys through the beam indirection
+            T = h.shape[0]
+            att = ops.attn_decode_rope_beam(qkv, self._rope_tab, cache.k(i), cache.v(i), cache.block_table, kv_len,
+                                            self.beam["beam_src"][:T], self.d_prompt[:T], H, D, cache.page_size,
+                                            max_kv_len)
         else:  # decode: RoPE + KV append happen inside the attention kernel
             att = ops.attn_decode_rope(qkv, self._rope_tab, cache.k(i), cache.v(i), cache.block_table, kv_len, H, D,
                                        cache.page_size, max_kv_len)
@@ -412,7 +461,7 @@ class LlamaEngine:
         return ops.gemm(h.index_select(0, last), self.lm_head, out_fp32=True, rms_eps=c.rms_norm_eps)
 
     # ------------------------------------------------------------------ decode
-    def _decode_body(self, B):
+    def _decode_body(self, B, beam=False):
         """One greedy token for slots 0..B-1: reads d_src/d_pos/d_len, leaves logits in d_logits,
         arg-max in d_next, and advances the device-side counters."""
         c = self.cfg
@@ -420,7 +469,7 @@ class LlamaEngine:
         self._rope_tab = ops.rope_table(self.d_pos[:B], c.head_dim, c.rope_theta, out=self.d_rope[:B])
         for i in range(c.num_hidden_layers):
             self._layer(i, h, self.d_pos[:B], self.d_bot[:B], None, kv_len=self.d_len[:B],
-                        max_kv_len=self.cache.max_seq_len)
+                        max_kv_len=self.cache.max_seq_len, beam=beam)
         ops.gemm(h, self.lm_head, out=self.d_logits[:B], out_fp32=True, rms_eps=c.rms_norm_eps)
 
     def _step_kernels(self, B, sampled=False):
@@ -433,6 +482,10 @@ class LlamaEngine:
             lib.vb200_set_pdl(prev)
 
     def _step_kernels_inner(self, B, sampled=False):
+        if sampled == "beam":
+            self._decode_body(B, beam=True)
+            self.beam_advance(self.d_logits[:B])
+            return
         self._decode_body(B)
         # token_log[b, d_len - d_prompt] = token; d_src = token; d_pos += 1; d_len += 1
         state = dict(next_src=self.d_src[:B], positions=self.d_pos[:B], kv_len=self.d_len[:B], token_log=self.token_log[:B],
@@ -456,6 +509,64 @@ class LlamaEngine:
         p = 1.0 if top_p is None else float(top_p)
         self.d_sample.copy_(ops.sample_params(max(float(temperature), 1e-6), k, p, seed))
 
+    def _beam_state(self):
+        if self.beam is None:
+            R, S, dev = self.max_batch, self.cache.max_seq_len, self.device
+            z = lambda *shape, dt=torch.int32: torch.zeros(shape, dtype=dt, device=dev)
+            self.beam = dict(beam_score=z(R, dt=torch.float32), parent=z(R), done=z(R), beam_src=z(R, S),
+                             hyp_score=z(R, dt=torch.float64), hyp_len=z(R), hyp_seq=z(R), hyp_count=z(R),
+                             hyp_ids=z(R, S, dt=torch.int64))
+            self.d_beam = torch.zeros((_beam.PARAMS.size,), dtype=torch.uint8, device=dev)
+            if dev.type == "cuda":
+                ops.reserve_beam_workspace(R, dev)
+        return self.beam
+
+    def _require_beam(self):
+        if self.beam is None or self.beam_k < 1:
+            raise RuntimeError("no beam search is set up on this engine: call start_beam() before beam steps")
+
+    def beam_advance(self, logits):
+        """The beam step over rows of fp32 logits with the start_beam parameters. A CUDA engine runs the kernel; a CPU
+        engine, which runs no kernels of this library, runs the host statement of the same contract (vitron_b200.beam)."""
+        self._require_beam()
+        R = logits.shape[0]
+        fn = ops.beam_advance if self.device.type == "cuda" else _beam.beam_advance
+        fn(logits, self.beam_k, self.d_beam, **{n: t[:R] for n, t in self.beam.items()}, next_src=self.d_src[:R],
+           positions=self.d_pos[:R], kv_len=self.d_len[:R], token_log=self.token_log[:R], prompt_len=self.d_prompt[:R])
+
+    def start_beam(self, logits, k, max_new_tokens, params):
+        """Beam search over the B prompts of the last prefill: logits [B, V] are its last-token logits, params a
+        beam.pack_params buffer. Rows b * k + j become the beams of request b, sharing its full prompt pages (the partial
+        last page is copied per beam); step 0 runs the beam kernel on the logits replicated to the k rows (generated
+        token 0). decode_steps(B * k, n, sampled="beam") then runs further steps."""
+        B = logits.shape[0]
+        R, lens = B * k, [int(x) for x in self._lens_host[:B]]
+        if not 1 <= k <= _beam.MAX_K:
+            raise ValueError(f"num_beams must be in 1..{_beam.MAX_K}, got {k}")
+        if R > self.max_batch:
+            raise ValueError(f"batch {B} x num_beams {k} = {R} rows > engine max_batch {self.max_batch}")
+        need = max(lens) + max_new_tokens
+        if need > self.cache.max_seq_len:
+            raise ValueError(f"prompt + max_new_tokens = {need} exceeds KV capacity {self.cache.max_seq_len}")
+        st = self._beam_state()
+        self.cache.fork(lens, k)
+        for r in range(R):
+            self.cache.reserve(r, lens[r // k] + max_new_tokens)
+        self.cache.sync_table()
+        self.beam_k = k
+        self.d_beam.copy_(params)
+        plen = torch.tensor(lens, dtype=torch.int32).repeat_interleave(k).to(self.device)
+        self.d_prompt[:R].copy_(plen)
+        self.d_len[:R].copy_(plen)            # kv_len - prompt_len = 0: the step below logs generated token 0
+        self.d_pos[:R].copy_(plen - 1)
+        self._lens_host = plen.tolist()
+        init = torch.full((B, k), -1e9, dtype=torch.float32)
+        init[:, 0] = 0.0
+        st["beam_score"][:R].copy_(init.reshape(-1))
+        for name in ("done", "hyp_count"):
+            st[name][:B].zero_()
+        self.beam_advance(logits.float().repeat_interleave(k, 0).contiguous())
+
     def start_decode(self, first_tokens, max_new_tokens):
         """first_tokens [B] int64: the token chosen from the prefill logits (already counted as
         generated token 0). Prepares device state for up to max_new_tokens-1 further steps."""
@@ -473,31 +584,37 @@ class LlamaEngine:
         self.d_src[:B] = first_tokens.to(torch.int32)
 
     def decode_steps(self, B, n, use_graph=True, sampled=False):
-        """Run n decode steps for slots 0..B-1 (no host sync): greedy, or sampled with the set_sampling parameters."""
+        """Run n decode steps for slots 0..B-1 (no host sync): greedy, sampled with the set_sampling parameters, or
+        (sampled="beam") beam steps over the B = requests x num_beams rows of start_beam."""
         if n <= 0:
             return
+        if sampled == "beam":
+            self._require_beam()
         if not use_graph or self.device.type != "cuda":   # (host-logic tests drive the same step un-graphed)
             for _ in range(n):
                 self._step_kernels(B, sampled)
             return
-        key = (B, bool(sampled))
+        key = (B, "beam", self.beam_k) if sampled == "beam" else (B, bool(sampled))
         if key not in self._graphs:
             # warm-up on a side stream (allocator + lazy init), then capture
             s = torch.cuda.Stream(device=self.device)
             s.wait_stream(torch.cuda.current_stream())
-            saved = [t.clone() for t in (self.d_src, self.d_pos, self.d_len, self.token_log)]
+            state = [self.d_src, self.d_pos, self.d_len, self.token_log]
+            if sampled == "beam":
+                state += list(self.beam.values())
+            saved = [t.clone() for t in state]
             with torch.cuda.stream(s):
                 self._step_kernels(B, sampled)
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
-            for t, sv in zip((self.d_src, self.d_pos, self.d_len, self.token_log), saved):
+            for t, sv in zip(state, saved):
                 t.copy_(sv)
             g = torch.cuda.CUDAGraph()
             l0 = ops.launch_count()
             with torch.cuda.graph(g):
                 self._step_kernels(B, sampled)
             self.launches_per_step = ops.launch_count() - l0
-            for t, sv in zip((self.d_src, self.d_pos, self.d_len, self.token_log), saved):
+            for t, sv in zip(state, saved):
                 t.copy_(sv)
             self._graphs[key] = g
         g = self._graphs[key]

@@ -9,7 +9,7 @@ import struct
 
 import torch
 
-from . import _lib
+from . import _lib, beam
 from .nf4 import NF4Weight
 from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_RELU, ACT_SILU, GLU_GEGLU, GLU_NONE,
                    GLU_SWIGLU, Epilogue, check)
@@ -511,6 +511,30 @@ def attn_decode_rope(qkv, table, k_pages, v_pages, block_table, kv_len, n_heads,
     return out
 
 
+def attn_decode_rope_beam(qkv, table, k_pages, v_pages, block_table, kv_len, beam_src, gen_start, n_heads, head_dim,
+                          page_size, max_kv_len, scale=None, out=None):
+    """attn_decode_rope for beam rows: key j >= gen_start[b] of row b is read from the pages of row beam_src[b, j]
+    (int32 [B, >= max_kv_len], rows index block_table); the new token's K / V still go to row b's own pages."""
+    lib = _lib.load()
+    B = qkv.shape[0]
+    _req(beam_src.dtype == torch.int32 and beam_src.dim() == 2 and beam_src.stride(1) == 1 and beam_src.shape[0] >= B
+         and gen_start.dtype == torch.int32 and gen_start.numel() >= B, "beam_src int32 [B, S], gen_start int32 [B]")
+    _req(beam_src.shape[1] >= max_kv_len, "beam_src must cover max_kv_len positions")
+    scale = 1.0 / math.sqrt(head_dim) if scale is None else scale
+    if out is None:
+        out = torch.empty((B, n_heads * head_dim), dtype=BF16, device=qkv.device)
+    need = lib.vb200_attn_decode_workspace_size(B, n_heads, head_dim, 32)
+    ws = workspace(need, qkv.device, "dec")
+    check(lib.vb200_attn_decode_rope_beam(qkv.data_ptr(), qkv.stride(0), table.data_ptr(), k_pages.data_ptr(),
+                                          v_pages.data_ptr(), block_table.data_ptr(), block_table.shape[1],
+                                          kv_len.data_ptr(), beam_src.data_ptr(), beam_src.stride(0),
+                                          gen_start.data_ptr(), out.data_ptr(), out.stride(0), B, n_heads, head_dim,
+                                          page_size, max_kv_len, float(scale), ws.data_ptr(), need, _stream()),
+          "vb200_attn_decode_rope_beam")
+    _launches[0] += 1
+    return out
+
+
 def row_rstd(x, eps):
     """fp32 [rows] = rsqrt(mean(x_row^2) + eps)."""
     lib = _lib.load()
@@ -584,6 +608,45 @@ def sample_advance(logits, params, out_idx=None, next_src=None, positions=None, 
                                    _ptr(prompt_len), _stream()), "vb200_sample_advance")
     _launches[0] += 1
     return out_idx
+
+
+def reserve_beam_workspace(rows, device):
+    """Pre-size the beam-step workspace for the most rows an engine will run (its address is baked into decode graphs)."""
+    return workspace(_lib.load().vb200_beam_workspace_size(rows), torch.device(device), "beam")
+
+
+def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
+                 next_src, positions, kv_len, token_log, prompt_len):
+    """One beam-search step for B = rows / k requests (contract in include/vitron_b200.h, statement in
+    vitron_b200.beam): parameters from the device buffer `params` (beam.pack_params), state updated in place."""
+    lib = _lib.load()
+    _req(logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1, "fp32 logits [B * k, V]")
+    R = logits.shape[0]
+    _req(k > 0 and R % k == 0, f"{R} rows are not a multiple of k = {k}")
+    _req(params.dtype == torch.uint8 and params.is_contiguous() and params.device == logits.device,
+         "params: uint8 beam parameter buffer on the logits' device")
+    _req(params.numel() == beam.PARAMS.size, f"params: {beam.PARAMS.size}-byte vb_beam_params buffer")
+    dev = logits.device
+    for name, t, dt in (("beam_src", beam_src, torch.int32), ("hyp_ids", hyp_ids, torch.int64),
+                        ("token_log", token_log, torch.int64)):
+        _req(t.dtype == dt and t.dim() == 2 and t.stride(1) == 1 and t.shape[0] >= R and t.device == dev,
+             f"{name}: {dt} [>= {R}, S] with unit inner stride on the logits' device")
+    for name, t, dt in (("beam_score", beam_score, torch.float32), ("hyp_score", hyp_score, torch.float64),
+                        ("parent", parent, torch.int32), ("done", done, torch.int32), ("hyp_len", hyp_len, torch.int32),
+                        ("hyp_seq", hyp_seq, torch.int32), ("hyp_count", hyp_count, torch.int32),
+                        ("next_src", next_src, torch.int32), ("positions", positions, torch.int32),
+                        ("kv_len", kv_len, torch.int32), ("prompt_len", prompt_len, torch.int32)):
+        _req(t.dtype == dt and t.dim() == 1 and t.is_contiguous() and t.numel() >= R and t.device == dev,
+             f"{name}: contiguous {dt} [>= {R}] on the logits' device")
+    need = lib.vb200_beam_workspace_size(R)
+    ws = workspace(need, logits.device, "beam")
+    check(lib.vb200_beam_advance(logits.data_ptr(), logits.stride(0), R // k, k, logits.shape[1], params.data_ptr(),
+                                 beam_score.data_ptr(), parent.data_ptr(), done.data_ptr(), beam_src.data_ptr(),
+                                 beam_src.stride(0), hyp_score.data_ptr(), hyp_len.data_ptr(), hyp_seq.data_ptr(),
+                                 hyp_count.data_ptr(), hyp_ids.data_ptr(), hyp_ids.stride(0), next_src.data_ptr(),
+                                 positions.data_ptr(), kv_len.data_ptr(), token_log.data_ptr(), token_log.stride(0),
+                                 prompt_len.data_ptr(), ws.data_ptr(), need, _stream()), "vb200_beam_advance")
+    _launches[0] += 1
 
 
 def patchify(pixels, patch, kpad):

@@ -14,7 +14,7 @@ from types import SimpleNamespace
 
 import torch
 
-from . import ops
+from . import beam, ops
 from .module_face import ModuleFace
 from .adapters import RegionExtractor, VisionProjector
 from .llama import LlamaConfig, LlamaEngine
@@ -492,20 +492,38 @@ class VitronLlamaForCausalLM(ModuleFace):
     @torch.no_grad()
     def generate(self, input_ids=None, images=None, regions=None, do_sample=False, temperature=1.0, top_p=None,
                  top_k=None, max_new_tokens=32, use_cache=True, stopping_criteria=None, attention_mask=None,
-                 eos_token_id=None, pad_token_id=None, inputs=None, sync_every=16, **kwargs):
+                 eos_token_id=None, pad_token_id=None, inputs=None, sync_every=16, num_beams=1, length_penalty=1.0,
+                 early_stopping=False, num_return_sequences=1, **kwargs):
         """Greedy (or sampled) decoding with the reference call signature
         (inference_image.py:53-61, app.py:562-571). Returns input_ids followed by the generated ids,
         like HF `generate` for decoder-only models.
 
         Both modes replay the same CUDA-graphed decode step; do_sample=True ends it with the device sampler
         (temperature, top_k, top_p, Philox draw) instead of the arg-max. Its seed is drawn once per call from torch's
-        default CPU generator, so `torch.manual_seed(s)` makes a sampled call reproducible."""
+        default CPU generator, so `torch.manual_seed(s)` makes a sampled call reproducible.
+
+        num_beams > 1 (with do_sample=False) is HF 4.31 beam search, stated in vitron_b200.beam: length_penalty divides
+        a hypothesis's summed log-probabilities by its whole length (prompt included) to that power, early_stopping is
+        True, False or "never", and the best num_return_sequences hypotheses of each request are returned, request-major,
+        as [B * num_return_sequences, input_len + gen_len]. The prompt (and its images) is prefilled once per request;
+        its beams share its KV pages, and the beam step runs on the device inside the graphed decode step, so the host
+        reads the done flags once per `sync_every` steps. With stopping_criteria the running beams are rebuilt after
+        every step (beams reorder their history), which syncs once per step. do_sample=True ignores num_beams, as
+        before: beam sampling is not implemented."""
         if input_ids is None:
             input_ids = inputs
         eos = self.config.eos_token_id if eos_token_id is None else eos_token_id
         pad = self.config.pad_token_id if pad_token_id is None else pad_token_id
         eos_set = set(eos if isinstance(eos, (list, tuple)) else [eos]) if eos is not None else set()
         B = input_ids.shape[0]
+        beam_search = num_beams > 1 and not do_sample
+        if beam_search:
+            if num_return_sequences > num_beams:
+                raise ValueError(f"num_return_sequences ({num_return_sequences}) has to be smaller or equal to "
+                                 f"num_beams ({num_beams})")
+            if B * num_beams > self.engine.max_batch:
+                raise ValueError(f"batch {B} x num_beams {num_beams} = {B * num_beams} rows > engine max_batch "
+                                 f"{self.engine.max_batch}")
         self._kv_segments = None          # the prefill and decode below overwrite the cache: every handle becomes stale
         if images is not None:
             _, _, am, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(
@@ -517,6 +535,10 @@ class VitronLlamaForCausalLM(ModuleFace):
         embeds, lens, _ = self._right_pad(embeds, am)
         eng = self.engine
         logits = eng.prefill(embeds, lens)
+        if beam_search:
+            eos_list = sorted(eos_set) if not isinstance(eos, (list, tuple)) else [int(e) for e in eos]
+            return self._beam_search(input_ids, logits, num_beams, num_return_sequences, length_penalty, early_stopping,
+                                     eos_list, pad, max_new_tokens, stopping_criteria, sync_every)
         if do_sample:
             seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64)) & (2 ** 64 - 1)
             eng.set_sampling(temperature, top_k, top_p, seed)
@@ -553,6 +575,45 @@ class VitronLlamaForCausalLM(ModuleFace):
         toks = eng.token_log[:B, :keep].cpu()
         gen = self._finalize(toks, done_at, pad)
         return torch.cat([input_ids, gen.to(input_ids.device)], 1)
+
+    def _beam_search(self, input_ids, logits, k, nrs, length_penalty, early_stopping, eos, pad, max_new_tokens,
+                     stopping_criteria, sync_every):
+        eng = self.engine
+        B, n_in = input_ids.shape
+        R = B * k
+        if pad is None:
+            pad = eos[0] if eos else 0
+        prm = dict(length_penalty=float(length_penalty), early_stopping=early_stopping, pad=int(pad), input_len=n_in,
+                   max_length=n_in + max_new_tokens, eos=eos)
+        eng.start_beam(logits, k, max_new_tokens, beam.pack_params(length_penalty, early_stopping, pad, n_in,
+                                                                   n_in + max_new_tokens, eos))
+        st = eng.beam
+        produced = 1
+        while produced < max_new_tokens:
+            if bool(st["done"][:B].cpu().all()):
+                break
+            if stopping_criteria is not None:
+                seq = torch.cat([input_ids.cpu().repeat_interleave(k, 0), self._running(produced, R)], 1)
+                if self._criteria_met(stopping_criteria, seq.to(input_ids.device)):
+                    break
+            n = 1 if stopping_criteria is not None else min(sync_every, max_new_tokens - produced)
+            eng.decode_steps(R, n, sampled="beam")
+            produced += n
+        done = st["done"][:B].cpu().tolist()
+        hs, hl, hq = st["hyp_score"][:R].cpu(), st["hyp_len"][:R].cpu(), st["hyp_seq"][:R].cpu()
+        counts, ids = st["hyp_count"][:B].cpu().tolist(), st["hyp_ids"][:R].cpu()
+        hyps = []
+        for b in range(B):
+            h = beam.Hypotheses(k, prm["length_penalty"], early_stopping, prm["max_length"])
+            h.slots = [dict(score=float(hs[b * k + s]), length=int(hl[b * k + s]), seq=int(hq[b * k + s]),
+                            ids=ids[b * k + s, :int(hl[b * k + s]) - n_in]) for s in range(counts[b])]
+            hyps.append(h)
+        gen = beam.finalize(hyps, done, st["beam_score"][:R].cpu(), self._running(produced, R), nrs, prm)
+        return torch.cat([input_ids.repeat_interleave(nrs, 0), gen.to(input_ids.device)], 1)
+
+    def _running(self, t, R):
+        eng = self.engine
+        return beam.running_ids(eng.beam["beam_src"][:R].cpu(), eng.token_log[:R].cpu(), eng.d_prompt[:R].cpu(), t)
 
     @staticmethod
     def _finalize(toks, done_at, pad):
