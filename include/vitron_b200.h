@@ -159,6 +159,8 @@ int vb200_groupnorm_nhwc(const void* x, const void* weight, const void* bias, vo
  * head dim is contiguous. kv_len: int32 [B] valid keys per batch or NULL. causal: key j visible
  * to query i iff j <= i + (Skv - Sq) and j < kv_len[b]. mask: uint8, non-zero = masked out, element strides
  * (mb, mh, mq) with keys contiguous, or NULL. Rows with every key masked produce zeros.
+ * The wgmma kernel loads whole 64-key blocks: V in [kv_len[b], Skv) and V under masked keys enter P·V with weight 0,
+ * so they must be finite (0 · NaN is NaN).
  * Replaces HF LlamaAttention / CLIPAttention eager bmm+softmax, xformers
  * memory_efficient_attention (i2vgen util.py:253-258; GLIGEN attention.py:176,247) and SEEM
  * multi_head_attention_forward (utils/attn.py:296-316). head_dim in {40,64,80,128,160}. */
