@@ -304,7 +304,8 @@ typedef struct vb_beam_params {
   int32_t eos[8];
 } vb_beam_params;          /* 64 bytes: 4 bytes of tail padding */
 
-/* workspace of vb200_beam_advance: [16 KB of arrival counters (B <= 4096) | candidates]; zero-filled ONCE by the caller */
+/* workspace of vb200_beam_advance and vb200_beam_sample_advance: [16 KB of arrival counters (B <= 4096) | candidates];
+ * zero-filled ONCE by the caller */
 size_t vb200_beam_workspace_size(int64_t rows);
 /* beam step of HF 4.31 beam_search for B requests x k beams (row r = b * k + j, 1 <= k <= 16, 2 <= n <= 49152, else
  * VB_ERR_UNSUPPORTED), stated in float64 in vitron_b200/beam.py:
@@ -327,6 +328,31 @@ int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, in
                        int64_t hyp_ld, int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
                        int64_t log_stride, const int32_t* prompt_len, void* workspace, size_t workspace_bytes,
                        cudaStream_t stream);
+/* beam-sampling step of HF 4.31 beam_sample (do_sample with num_beams = k) for B searches x k beams, stated in float64
+ * in vitron_b200/beam.py: vb200_beam_advance's arguments, limits and bookkeeping, plus sampling parameters in DEVICE
+ * memory (temperature, top_k, top_p, seed of vb_sample_params). Per search b, step t = kv_len - prompt_len of row b * k:
+ *   w[r, i] = (log_softmax(logits[r])[i] + beam_score[r]) / T (fp32; NaN counts as -inf), the warpers applied AFTER
+ *   adding the running beam scores, as 4.31 does (its beam_sample starts every beam at score 0). Temperature compounds
+ *   into the carried scores: at T < 1 a long search's w leaves the fp32 range and becomes -inf, where 4.31 raises;
+ *   a search with no entry above -inf has no draws, and its beams continue their own rows with pad and score -1e9;
+ *   per row, the kept set of vb200_sample_advance's top-k and top-p over w (within a row, w is the sampler's logit / T
+ *   plus a constant: the kernel cuts on (logit - max logit) / T), with top-k at least 2 when on and top-p keeping every
+ *   entry with fewer than 2 strictly larger kept ones (min_tokens_to_keep = 2);
+ *   draws: key = w - log(-log U) over the kept entries with w > -inf, U = (2 * (x >> 9) + 1) * 2^-24 in (0, 1), x =
+ *   word f % 4 of Philox4x32-10(counter (t, b, f / 4, 1), key (seed_lo, seed_hi)), f = j * n + i the flat index; the
+ *   2k largest keys (ties to the lower flat index) are the draws without replacement (torch.multinomial as an
+ *   exponential race); entries whose probability underflows to 0 rank after every positive one and are drawn in key
+ *   order where 4.31 raises; fewer than 2k keyed entries give fewer draws;
+ *   the draws are ranked by w (descending, ties to the lower flat index) and run through vb200_beam_advance's scorer
+ *   with w as the candidate score: new beam scores and hypothesis scores are warped scores.
+ * Deterministic: bit-identical outputs whatever the order in which the rows' CTAs finish. */
+int vb200_beam_sample_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                              const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
+                              int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len, int32_t* hyp_seq,
+                              int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld, int32_t* next_src,
+                              int32_t* positions, int32_t* kv_len, int64_t* token_log, int64_t log_stride,
+                              const int32_t* prompt_len, void* workspace, size_t workspace_bytes,
+                              const vb_sample_params* sample_params, cudaStream_t stream);
 
 /* ---- vision / diffusion glue (vision.cu) ----------------------------------------------------
  * patchify: NCHW pixels -> [nb*gh*gw, kpad] rows ordered (c, py, px) for the patch-embed GEMM

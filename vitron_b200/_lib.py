@@ -76,6 +76,8 @@ SIGNATURES = {
     "vb200_beam_workspace_size": (_sz, [_i64]),
     "vb200_beam_advance": (_i32, [_p, _i64, _i64, _i64, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64, _p, _p,
                                   _p, _p, _i64, _p, _p, _sz, _p]),
+    "vb200_beam_sample_advance": (_i32, [_p, _i64, _i64, _i64, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64,
+                                         _p, _p, _p, _p, _i64, _p, _p, _sz, _p, _p]),
     "vb200_patchify": (_i32, [_p, _i32, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p]),
     "vb200_vit_embed_ln": (_i32, [_p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _f, _p]),
     "vb200_upsample2x_nhwc": (_i32, [_p, _p, _i64, _i64, _i64, _i64, _p]),

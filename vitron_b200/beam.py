@@ -26,6 +26,41 @@ GPU tests compare the kernel with it. The rules, in order:
    request (highest score, the latest added among equals, as 4.31's stable sort + pop), pads with pad and appends
    eos[0] (pad when there is no EOS id) where a hypothesis is shorter than the output, which is
    min(longest + 1, max_length) positions wide.
+
+Beam sampling (vb200_beam_sample_advance, `generate(do_sample=True, num_beams=k)`) restates 4.31's
+`GenerationMixin.beam_sample` and the `is_beam_sample_gen_mode` branch of `GenerationMixin.generate`
+(transformers/generation/utils.py at v4.31.0). Rules 4-8 hold as above; rules 1-3 become, per search b, step t:
+
+1s. Initial beam scores are 0 for every beam. 4.31's beam_sample initialises
+        beam_scores = torch.zeros((batch_size, num_beams), dtype=torch.float, device=input_ids.device)
+        beam_scores = beam_scores.view((batch_size * num_beams,))
+    without beam_search's `beam_scores[:, 1:] = -1e9`: step 0 draws its 2k candidates from k identical live rows, so
+    two beams may take the same token (ties in w go to the lower flat index, i.e. the lower beam).
+2s. c = log_softmax(fp32 logits[r]) + beam_score[r] (`next_token_scores + beam_scores[:, None]`), then the logits warpers
+    on the cumulative c ("intentionally applied after adding running beam scores"): TemperatureLogitsWarper w = c / T,
+    TopKLogitsWarper(max(top_k, 2)) and TopPLogitsWarper(top_p, min_tokens_to_keep=2) (`_get_logits_warper` passes
+    min_tokens_to_keep = 2 when num_beams > 1); removed entries become -inf. top_k None / 0 is off, as in the sampled
+    path. Within a row top-k and top-p see w up to a constant, so they are vitron_b200.sampling's value-based cuts of
+    the sampler (ties at a cut stay together) with "at least the 2 largest kept" added; 4.31 keeps the last 2 of its
+    ascending sort, which differs only in tie order. w is an fp32 value, as in 4.31: a w below the fp32 range is -inf.
+    Temperature compounds, |w_t| ~ (|s| + |w_{t-1}|) / T, so at T < 1 a long search's scores leave the fp32 range (at
+    T = 0.2 after roughly 55 steps). 4.31 then raises (softmax of an all -inf row is NaN, and multinomial rejects it);
+    here a search whose entries are all -inf has no draws, so by rule 4 its k beams continue their own rows with pad
+    and score -1e9, and the next step's scores are finite again.
+3s. `probs = softmax(w.view(B, k * V))`, `torch.multinomial(probs, 2k)` without replacement, then the drawn scores are
+    sorted descending. The draw is stated as torch's own algorithm, an exponential race, in the log domain:
+    key = w - log(-log U) over the entries with w > -inf; the 2k largest keys (ties to the lower flat index f = j * V +
+    token) are the draws. U = (2 * (x >> 9) + 1) * 2^-24 in (0, 1), x = word f % 4 of Philox4x32-10(counter
+    (t, b, f // 4, 1), key (seed low 32 bits, seed high 32 bits)). The draws are ranked by w, descending, ties to the
+    lower flat index (torch.sort leaves tie order open), and go through rules 4-7 with w as the candidate score: the new
+    beam scores and the hypotheses' sum_logprobs are warped scores. Entries whose fp32 probability underflows to 0
+    (e.g. the pad beams of rule 4 at -1e9 next to live ones) rank after every positive one and are drawn in key order
+    where 4.31 raises ("not enough non-negative category to sample"); fewer than 2k entries with w > -inf give fewer
+    draws, handled as rule 4's missing beams.
+5s. num_return_sequences = r runs r independent searches per prompt: 4.31 builds
+    `BeamSearchScorer(batch_size=batch_size * num_return_sequences, ...)` and expands the input by
+    `num_beams * num_return_sequences`, and finalize keeps each search's best hypothesis, so the output is [B * r, L]
+    in request-major order (search b * r + i samples prompt b).
 """
 import struct
 
@@ -126,15 +161,80 @@ def process(cands, k, V, hyps, t, prm):
             children.append((j, tok, score))
     while len(children) < k:
         children.append((len(children), prm["pad"], -1e9))
-    return children, added, hyps.is_done(cands[0][0], prm["input_len"] + t)
+    return children, added, hyps.is_done(cands[0][0] if cands else float("-inf"), prm["input_len"] + t)
 
 
 def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
                  next_src, positions, kv_len, token_log, prompt_len):
     """Same arguments and bookkeeping as ops.beam_advance, on host tensors."""
-    prm = unpack_params(params)
-    R, V = logits.shape
     lsm = log_softmax64(logits)
+
+    def cands(b, r0, t):
+        return top_candidates(lsm[r0:r0 + k] + beam_score[r0:r0 + k].double().cpu()[:, None], k)
+    _advance(cands, logits.shape, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
+             hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
+
+
+def warped_scores(logits, beam_score, temperature):
+    """Rule 2s up to the cuts: w = (log_softmax(logits) + beam_score) / T, float64 [R, V]; a w that fp32 cannot hold is
+    -inf."""
+    w = (log_softmax64(logits) + beam_score.double().cpu()[:, None]) / float(temperature)
+    return torch.where(torch.isinf(w.float()), torch.full_like(w, float("-inf")), w)
+
+
+def warp_kept(w, top_k, top_p):
+    """Rule 2s's cuts per row of w: (kept bool [R, V], near bool [R]: a top-p fraction within 1e-5 of top_p)."""
+    from .sampling import sample_support
+    kept, _, near = sample_support(w, 1.0, max(int(top_k), 2) if top_k > 0 else 0, float(top_p), min_keep=2)
+    return kept & (w > float("-inf")), near
+
+
+def gumbel(seed, t, b, flat):
+    """Rule 3s's noise -log(-log U) of the flat indices `flat` (int array) of search b at step t, float64."""
+    from .sampling import philox4x32_10
+    flat = np.asarray(flat, dtype=np.uint64)
+    ctr = np.stack([np.full_like(flat, t & 0xFFFFFFFF), np.full_like(flat, b), flat >> np.uint64(2),
+                    np.ones_like(flat)], -1)
+    key = np.broadcast_to(np.array([seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF], dtype=np.uint64), ctr.shape[:-1] + (2,))
+    x = np.take_along_axis(philox4x32_10(ctr, key), (flat & np.uint64(3)).astype(np.int64)[..., None], -1)[..., 0]
+    u = (2.0 * (x >> np.uint64(9)).astype(np.float64) + 1.0) * 2.0 ** -24
+    return -np.log(-np.log(u))
+
+
+def sample_draws(w, kept, k, b, t, seed):
+    """Rule 3s for one search: w / kept [k, V]. Returns (draws [(w, flat)] ranked by w, keys of every keyed entry
+    sorted descending)."""
+    V = w.shape[1]
+    flat = np.nonzero(kept.reshape(-1).numpy())[0]
+    if flat.size == 0:
+        return [], np.zeros(0)
+    key = w.reshape(-1).numpy()[flat] + gumbel(seed, t, b, flat)
+    order = np.lexsort((flat, -key))
+    drawn = [(float(w.reshape(-1)[f]), int(f)) for f in flat[order[:2 * k]]]
+    drawn.sort(key=lambda c: (-c[0], c[1]))
+    assert all(0 <= f < k * V for _, f in drawn)
+    return drawn, key[order]
+
+
+def beam_sample_advance(logits, k, params, sample_params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq,
+                        hyp_count, hyp_ids, next_src, positions, kv_len, token_log, prompt_len):
+    """Same arguments and bookkeeping as ops.beam_sample_advance, on host tensors."""
+    from .ops import SAMPLE_PARAMS
+    temperature, top_k, top_p, _, seed = SAMPLE_PARAMS.unpack(sample_params.cpu().numpy().tobytes())
+    w = warped_scores(logits, beam_score, temperature)
+    kept, _ = warp_kept(w, top_k, top_p)
+
+    def cands(b, r0, t):
+        return sample_draws(w[r0:r0 + k], kept[r0:r0 + k], k, b, t, seed)[0]
+    _advance(cands, logits.shape, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
+             hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
+
+
+def _advance(cands_of, shape, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
+             hyp_ids, next_src, positions, kv_len, token_log, prompt_len):
+    """Rules 4-7 and the bookkeeping of one step; cands_of(b, r0, t) gives request b's ranked (score, flat) candidates."""
+    prm = unpack_params(params)
+    R, V = shape
     for b in range(R // k):
         r0 = b * k
         t, P = int(kv_len[r0]) - int(prompt_len[r0]), int(prompt_len[r0])
@@ -144,8 +244,7 @@ def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_scor
             hyps = Hypotheses(k, prm["length_penalty"], prm["early_stopping"], prm["max_length"])
             hyps.slots = [dict(score=float(hyp_score[r0 + s]), length=int(hyp_len[r0 + s]), seq=int(hyp_seq[r0 + s]))
                           for s in range(int(hyp_count[b]))]
-            scores = lsm[r0:r0 + k] + beam_score[r0:r0 + k].double().cpu()[:, None]
-            children, added, is_done = process(top_candidates(scores, k), k, V, hyps, t, prm)
+            children, added, is_done = process(cands_of(b, r0, t), k, V, hyps, t, prm)
             for s, h in enumerate(hyps.slots):
                 hyp_score[r0 + s], hyp_len[r0 + s], hyp_seq[r0 + s] = h["score"], h["length"], h["seq"]
             hyp_count[b] = len(hyps.slots)

@@ -506,6 +506,123 @@ __device__ T block_exclusive_scan(T v, T* buf, T* total) {
   return r;
 }
 
+// Shared-memory scratch of the radix selects below (one CTA of SMP_THREADS threads).
+struct SmpScratch {
+  uint32_t* h_cnt;               // [SMP_BINS]
+  unsigned long long* h_mass;    // [SMP_BINS]
+  unsigned long long* s_u64;     // [33]
+  uint32_t* s_bin;
+  unsigned long long* s_above;
+};
+
+// p_i = exp(z_i - max z), z = v / T, as fixed point; the maximum itself is exactly 1 (also for +-inf)
+__device__ __forceinline__ unsigned long long smp_mass(float v, float mx, float temp) {
+  const float p = v == mx ? 1.f : expf((v - mx) / temp);
+  return __float2ull_rn(p * SMP_FIX);
+}
+
+// 64-bit add to shared memory as two native 32-bit atomics, the low word's carry going to the high word: the 64-bit
+// shared atomicAdd is a compare-and-swap loop, which a bin many entries fall into turns into long retry chains. The sum
+// is exact, so the order of the adds does not matter.
+__device__ __forceinline__ void smp_add_u64(unsigned long long* a, unsigned long long v) {
+  uint32_t* w = reinterpret_cast<uint32_t*>(a);
+  const uint32_t lo = static_cast<uint32_t>(v), hi = static_cast<uint32_t>(v >> 32);
+  const uint32_t old = atomicAdd(w, lo);
+  const uint32_t up = hi + (old + lo < old ? 1u : 0u);
+  if (up) atomicAdd(w + 1, up);
+}
+
+// One radix level over the kept keys (order_key >= thr) of srow[0, n) whose bits above `shift + width` equal `prefix`:
+// histogram of the digit, then the lowest non-empty bin whose "before" value (count / mass of the kept keys in strictly
+// higher bins, plus `above`) is still below `limit`. Returns that bin; *s_above gets its "before" value.
+__device__ uint32_t smp_radix_level(const float* srow, int n, uint32_t thr, float mx, float temp, const SmpScratch& sc,
+                                    uint32_t prefix, uint32_t himask, int shift, uint32_t dmask, bool by_mass,
+                                    unsigned long long above, unsigned long long limit) {
+  const int tid = threadIdx.x;
+  for (int i = tid; i < SMP_BINS; i += SMP_THREADS) { sc.h_cnt[i] = 0; sc.h_mass[i] = 0; }
+  if (tid == 0) *sc.s_bin = SMP_BINS;
+  __syncthreads();
+  for (int i = tid; i < n; i += SMP_THREADS) {
+    const float v = srow[i];
+    const uint32_t key = order_key(v);
+    if (key >= thr && (key & himask) == prefix) {
+      const uint32_t d = (key >> shift) & dmask;
+      atomicAdd(&sc.h_cnt[d], 1u);
+      if (by_mass) smp_add_u64(&sc.h_mass[d], smp_mass(v, mx, temp));
+    }
+  }
+  __syncthreads();
+  // thread t owns bins hi = 2047 - 2t and hi - 1; scan in descending bin order
+  const int hi = SMP_BINS - 1 - 2 * tid, lo = hi - 1;
+  const unsigned long long w_hi = by_mass ? sc.h_mass[hi] : sc.h_cnt[hi], w_lo = by_mass ? sc.h_mass[lo] : sc.h_cnt[lo];
+  unsigned long long tot;
+  const unsigned long long before_hi = above + block_exclusive_scan(w_hi + w_lo, sc.s_u64, &tot);
+  const unsigned long long before_lo = before_hi + w_hi;
+  if (sc.h_cnt[lo] > 0 && before_lo < limit) atomicMin(sc.s_bin, static_cast<uint32_t>(lo));
+  else if (sc.h_cnt[hi] > 0 && before_hi < limit) atomicMin(sc.s_bin, static_cast<uint32_t>(hi));
+  __syncthreads();
+  const uint32_t sel = *sc.s_bin;
+  if (sel == static_cast<uint32_t>(lo)) *sc.s_above = before_lo;
+  if (sel == static_cast<uint32_t>(hi)) *sc.s_above = before_hi;
+  __syncthreads();
+  return sel;
+}
+
+// the cut key: radix descent over the three digits (bits 31..21, 20..10, 9..0)
+__device__ uint32_t smp_select_key(const float* srow, int n, uint32_t thr, float mx, float temp, const SmpScratch& sc,
+                                   bool by_mass, unsigned long long limit) {
+  uint32_t prefix = 0, himask = 0;
+  unsigned long long above = 0;
+#pragma unroll 1
+  for (int lvl = 0; lvl < 3; ++lvl) {
+    const int shift = lvl == 0 ? 21 : lvl == 1 ? 10 : 0;
+    const uint32_t d = smp_radix_level(srow, n, thr, mx, temp, sc, prefix, himask, shift, lvl == 2 ? 1023u : 2047u,
+                                       by_mass, above, limit);
+    above = *sc.s_above;
+    prefix |= d << shift;
+    himask = lvl == 0 ? 0xFFE00000u : 0xFFFFFC00u;
+  }
+  return prefix;
+}
+
+__device__ unsigned long long smp_kept_mass(const float* srow, int n, uint32_t thr, float mx, float temp,
+                                            const SmpScratch& sc) {
+  unsigned long long m = 0, tot;
+  for (int i = threadIdx.x; i < n; i += SMP_THREADS) {
+    const float v = srow[i];
+    if (order_key(v) >= thr) m += smp_mass(v, mx, temp);
+  }
+  block_exclusive_scan(m, sc.s_u64, &tot);
+  return tot;
+}
+
+// The warpers of the staged row srow[0, n) (values v, z = v / temp, mx = max v, `valid` = non-NaN count). Returns thr:
+// the kept set is {i : order_key(v_i) >= thr}; *total gets its mass.
+//   top-k: the k-th largest kept key; ties at it stay (count of strictly larger keys < k);
+//   top-p: keep i iff the kept mass of strictly larger keys is < top_p * total; the maximum always stays, and with
+//   min_keep = 2 so does every key with fewer than 2 strictly larger kept keys (TopPLogitsWarper's min_tokens_to_keep).
+__device__ uint32_t smp_warp(const float* srow, int n, uint32_t valid, float mx, float temp, int top_k, float top_p,
+                             int min_keep, const SmpScratch& sc, unsigned long long* total) {
+  uint32_t thr = 1u;   // thr = 1 drops only the NaNs
+  if (top_k > 0 && static_cast<uint32_t>(top_k) < valid)
+    thr = smp_select_key(srow, n, thr, mx, temp, sc, false, static_cast<unsigned long long>(top_k));
+  *total = smp_kept_mass(srow, n, thr, mx, temp, sc);
+  if (top_p < 1.f) {
+    uint32_t cut;
+    if (top_p <= 0.f) {
+      cut = order_key(mx);
+    } else {
+      const unsigned long long limit =
+          static_cast<unsigned long long>(ceil(static_cast<double>(top_p) * static_cast<double>(*total)));
+      cut = smp_select_key(srow, n, thr, mx, temp, sc, true, limit);
+    }
+    if (min_keep > 1) cut = min(cut, smp_select_key(srow, n, thr, mx, temp, sc, false, min_keep));
+    thr = cut;
+    *total = smp_kept_mass(srow, n, thr, mx, temp, sc);
+  }
+  return thr;
+}
+
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 sample_advance_kernel(const float* __restrict__ logits, long long ld, int n, const vb_sample_params* __restrict__ prm,
                       int64_t* __restrict__ out_idx, int32_t* __restrict__ next_src, int32_t* __restrict__ positions,
@@ -561,86 +678,11 @@ sample_advance_kernel(const float* __restrict__ logits, long long ld, int n, con
 
   int tok = 0;   // a row without a number samples token 0, like the arg-max
   if (valid > 0) {
-    const float temp = prm->temperature, top_p = prm->top_p;
-    const int top_k = prm->top_k;
-    // p_i = exp(z_i - max z), z = logit / T, as fixed point; the maximum itself is exactly 1 (also for +-inf)
-    auto mass_of = [&](float v) -> unsigned long long {
-      const float p = v == mx ? 1.f : expf((v - mx) / temp);
-      return __float2ull_rn(p * SMP_FIX);
-    };
-    uint32_t thr = 1u;   // kept set = {i : order_key(logit_i) >= thr}; thr = 1 drops only the NaNs
-
-    // One radix level over the kept keys whose bits above `shift + width` equal `prefix`: histogram of the digit, then
-    // the lowest non-empty bin whose "before" value (count / mass of the kept keys in strictly higher bins, plus `above`)
-    // is still below `limit`. Returns that bin; s_above gets its "before" value.
-    auto radix_level = [&](uint32_t prefix, uint32_t himask, int shift, uint32_t dmask, bool by_mass,
-                           unsigned long long above, unsigned long long limit) -> uint32_t {
-      for (int i = tid; i < SMP_BINS; i += SMP_THREADS) { h_cnt[i] = 0; h_mass[i] = 0; }
-      if (tid == 0) s_bin = SMP_BINS;
-      __syncthreads();
-      for (int i = tid; i < n; i += SMP_THREADS) {
-        const float v = srow[i];
-        const uint32_t key = order_key(v);
-        if (key >= thr && (key & himask) == prefix) {
-          const uint32_t d = (key >> shift) & dmask;
-          atomicAdd(&h_cnt[d], 1u);
-          if (by_mass) atomicAdd(&h_mass[d], mass_of(v));
-        }
-      }
-      __syncthreads();
-      // thread t owns bins hi = 2047 - 2t and hi - 1; scan in descending bin order
-      const int hi = SMP_BINS - 1 - 2 * tid, lo = hi - 1;
-      const unsigned long long w_hi = by_mass ? h_mass[hi] : h_cnt[hi], w_lo = by_mass ? h_mass[lo] : h_cnt[lo];
-      unsigned long long tot;
-      const unsigned long long before_hi = above + block_exclusive_scan(w_hi + w_lo, s_u64, &tot);
-      const unsigned long long before_lo = before_hi + w_hi;
-      if (h_cnt[lo] > 0 && before_lo < limit) atomicMin(&s_bin, static_cast<uint32_t>(lo));
-      else if (h_cnt[hi] > 0 && before_hi < limit) atomicMin(&s_bin, static_cast<uint32_t>(hi));
-      __syncthreads();
-      const uint32_t sel = s_bin;
-      if (sel == static_cast<uint32_t>(lo)) s_above = before_lo;
-      if (sel == static_cast<uint32_t>(hi)) s_above = before_hi;
-      __syncthreads();
-      return sel;
-    };
-    // the cut key: radix descent over the three digits (bits 31..21, 20..10, 9..0)
-    auto select_key = [&](bool by_mass, unsigned long long limit) -> uint32_t {
-      uint32_t prefix = 0, himask = 0;
-      unsigned long long above = 0;
-#pragma unroll 1
-      for (int lvl = 0; lvl < 3; ++lvl) {
-        const int shift = lvl == 0 ? 21 : lvl == 1 ? 10 : 0;
-        const uint32_t d = radix_level(prefix, himask, shift, lvl == 2 ? 1023u : 2047u, by_mass, above, limit);
-        above = s_above;
-        prefix |= d << shift;
-        himask = lvl == 0 ? 0xFFE00000u : 0xFFFFFC00u;
-      }
-      return prefix;
-    };
-    auto kept_mass = [&]() -> unsigned long long {
-      unsigned long long m = 0, tot;
-      for (int i = tid; i < n; i += SMP_THREADS) {
-        const float v = srow[i];
-        if (order_key(v) >= thr) m += mass_of(v);
-      }
-      block_exclusive_scan(m, s_u64, &tot);
-      return tot;
-    };
-
-    // top-k: the k-th largest kept key; ties at it stay (count of strictly larger keys < k)
-    if (top_k > 0 && static_cast<uint32_t>(top_k) < valid) thr = select_key(false, static_cast<unsigned long long>(top_k));
-    unsigned long long total = kept_mass();
-    // top-p: keep i iff the kept mass of strictly larger keys is < top_p * total; the maximum always stays
-    if (top_p < 1.f) {
-      if (top_p <= 0.f) {
-        thr = order_key(mx);
-      } else {
-        const unsigned long long limit =
-            static_cast<unsigned long long>(ceil(static_cast<double>(top_p) * static_cast<double>(total)));
-        thr = select_key(true, limit);
-      }
-      total = kept_mass();
-    }
+    const float temp = prm->temperature;
+    const SmpScratch sc{h_cnt, h_mass, s_u64, &s_bin, &s_above};
+    unsigned long long total;
+    const uint32_t thr = smp_warp(srow, n, valid, mx, temp, prm->top_k, prm->top_p, 1, sc, &total);
+    auto mass_of = [&](float v) { return smp_mass(v, mx, temp); };
 
     // draw: u = (philox[0] >> 8) * 2^-24; first kept index (vocabulary order) whose inclusive prefix mass > u * total.
     // prefix > u * total  <=>  prefix > floor(a * total / 2^24) for integer prefix, a = philox[0] >> 8
@@ -705,6 +747,33 @@ __device__ __forceinline__ bool bm_better(float sa, int ia, float sb, int ib) {
   return sa > sb || (sa == sb && ia < ib);
 }
 
+// The history-reorder stage buffer. The sampling variant overlays the radix selects' mass histogram on it: the selects
+// finish before the reorder starts, and the row (<= 192 KB) plus both would not fit an SM's shared memory.
+template <bool SAMPLE>
+struct BmStage {
+  typedef int32_t type[BM_MAX_K][BM_STAGE];
+  __device__ static type& get(type& s) { return s; }
+};
+template <>
+struct BmStage<true> {
+  union type {
+    int32_t stage[BM_MAX_K][BM_STAGE];
+    unsigned long long mass[SMP_BINS];
+  };
+  __device__ static int32_t (&get(type& s))[BM_MAX_K][BM_STAGE] { return s.stage; }
+};
+
+// Gumbel noise of flat index f of search b at step t: U = (2 * (x >> 9) + 1) * 2^-24 in (0, 1), x = word f % 4 of
+// Philox4x32-10(counter (t, b, f / 4, 1), key (seed_lo, seed_hi)); the noise is -log(-log U).
+__device__ __forceinline__ float bm_gumbel(uint32_t x) {
+  const float u = static_cast<float>(2u * (x >> 9) + 1u) * 5.9604644775390625e-8f;   // 2^-24
+  return -logf(-logf(u));
+}
+
+// SAMPLE = false: beam search. SAMPLE = true: beam sampling (HF 4.31 beam_sample): the rows' scores are warped
+// (temperature, top-k, top-p with 2 kept) and 2k candidates per request are drawn without replacement as the top 2k of
+// key = w + Gumbel noise; they are then ranked by warped score and go through the same scorer.
+template <bool SAMPLE>
 __global__ void __launch_bounds__(BM_THREADS, 1)
 beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k, const vb_beam_params* __restrict__ prm,
                     float* __restrict__ beam_score, int32_t* __restrict__ parent, int32_t* __restrict__ done,
@@ -713,7 +782,8 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
                     int64_t* __restrict__ hyp_ids, int hyp_ld, int32_t* __restrict__ next_src,
                     int32_t* __restrict__ positions, int32_t* __restrict__ kv_len, int64_t* __restrict__ token_log,
                     int log_stride, const int32_t* __restrict__ prompt_len, float* __restrict__ cand_s,
-                    int32_t* __restrict__ cand_i, int32_t* __restrict__ counters) {
+                    int32_t* __restrict__ cand_i, int32_t* __restrict__ counters,
+                    const vb_sample_params* __restrict__ sprm, float* __restrict__ cand_w) {
   extern __shared__ float srow[];
   __shared__ float s_f[32];
   __shared__ int s_i[32];
@@ -725,7 +795,8 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
   __shared__ int t_i[2 * BM_MAX_K];
   __shared__ int c_par[BM_MAX_K], c_tok[BM_MAX_K], h_src[BM_MAX_K];
   __shared__ float c_sc[BM_MAX_K];
-  __shared__ int32_t stage[BM_MAX_K][BM_STAGE];
+  __shared__ typename BmStage<SAMPLE>::type stage_buf;
+  auto& stage = BmStage<SAMPLE>::get(stage_buf);
   const int r = blockIdx.x, b = r / k, j = r % k, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int k2 = 2 * k;
   pdl_wait();      // logits, scores and the decode state come from the predecessors
@@ -763,7 +834,44 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
   const float bsc = beam_score[r];
   // candidate score = log_softmax + beam score, as torch computes it: (x - max) - log(sum exp(x - max))
   auto score_of = [&](int i) -> float { return mx == -INFINITY ? -INFINITY : ((srow[i] - mx) - logz) + bsc; };
-
+  float temp = 1.f;
+  if constexpr (SAMPLE) {
+    // ---- the warpers' kept set, cut on d = (x - max x) / T: within the row the warped scores w are d plus a constant,
+    // and d spreads over the float exponents as the sampler's logits do (w of a flat row shares one exponent, and its
+    // histogram atomics would all hit a few bins). Then srow[i] = w_i + Gumbel noise of (b, flat index) over the kept
+    // entries with w > -inf, -inf elsewhere.
+    __shared__ uint32_t h_cnt[SMP_BINS];
+    __shared__ unsigned long long s_u64[33];
+    __shared__ uint32_t s_bin;
+    __shared__ unsigned long long s_above;
+    temp = sprm->temperature;
+    uint32_t thr = 0xFFFFFFFFu;   // a row without a number keeps nothing
+    if (mx > -INFINITY) {
+      for (int i = tid; i < n; i += BM_THREADS) srow[i] = (srow[i] - mx) / temp;
+      __syncthreads();
+      const SmpScratch sc{h_cnt, stage_buf.mass, s_u64, &s_bin, &s_above};
+      const int top_k = sprm->top_k > 0 ? max(sprm->top_k, 2) : 0;
+      unsigned long long total;
+      thr = smp_warp(srow, n, static_cast<uint32_t>(n), 0.f, 1.f, top_k, sprm->top_p, 2, sc, &total);
+    }
+    const uint32_t t = static_cast<uint32_t>(kv_len[b * k] - prompt_len[b * k]);
+    const unsigned long long seed = sprm->seed;
+    const uint32_t f0 = static_cast<uint32_t>(j) * n, g0 = f0 >> 2, g1 = (f0 + n - 1) >> 2;
+    for (uint32_t g = g0 + tid; g <= g1; g += BM_THREADS) {
+      const uint4 x = philox4x32_10(make_uint4(t, static_cast<uint32_t>(b), g, 1u), static_cast<uint32_t>(seed),
+                                    static_cast<uint32_t>(seed >> 32));
+      const uint32_t xw[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int i = static_cast<int>(4 * g + q - f0);
+        if (4 * g + q < f0 || i >= n) continue;
+        const bool keep = order_key(srow[i]) >= thr;
+        const float w = ((((row[i] - mx) - logz) + bsc) / temp);   // the candidate score below, computed the same way
+        srow[i] = (keep && w > -INFINITY) ? w + bm_gumbel(xw[q]) : -INFINITY;
+      }
+    }
+    __syncthreads();
+  }
   // ---- this row's top 2k
   float ps = INFINITY;
   int pi = -1;           // the last candidate this thread supplied: the next one must come after it
@@ -773,7 +881,9 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
     my_s = -INFINITY;
     my_i = INT_MAX;
     for (int i = tid; i < n; i += BM_THREADS) {
-      const float sv = score_of(i);
+      float sv;
+      if constexpr (SAMPLE) sv = srow[i];
+      else sv = score_of(i);
       if ((sv < ps || (sv == ps && i > pi)) && bm_better(sv, i, my_s, my_i)) { my_s = sv; my_i = i; }
     }
   };
@@ -805,7 +915,14 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
     const int wi = s_wi;
     if (tid == 0) {
       cand_s[r * 2 * BM_MAX_K + q] = ws;
-      cand_i[r * 2 * BM_MAX_K + q] = wi == INT_MAX ? BM_SENTINEL + r * 2 * BM_MAX_K + q : j * n + wi;
+      if constexpr (SAMPLE) {   // an entry without a key is no draw; a draw carries its warped score, recomputed from
+                                // its logit exactly as it was staged
+        const bool none = wi == INT_MAX || ws == -INFINITY;
+        cand_i[r * 2 * BM_MAX_K + q] = none ? BM_SENTINEL + r * 2 * BM_MAX_K + q : j * n + wi;
+        cand_w[r * 2 * BM_MAX_K + q] = none ? -INFINITY : ((((row[wi] - mx) - logz) + bsc) / temp);
+      } else {
+        cand_i[r * 2 * BM_MAX_K + q] = wi == INT_MAX ? BM_SENTINEL + r * 2 * BM_MAX_K + q : j * n + wi;
+      }
     }
     if (wi != INT_MAX && wi % BM_THREADS == tid) { ps = ws; pi = wi; rescan(); }
   }
@@ -820,16 +937,42 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
   if (!s_last) return;
   __threadfence();
   const int r0 = b * k, nc = k * k2;
-  for (int c = tid; c < nc; c += BM_THREADS) {
-    const int idx = (r0 + c / k2) * 2 * BM_MAX_K + c % k2;
-    m_s[c] = __ldcg(&cand_s[idx]);
-    m_i[c] = __ldcg(&cand_i[idx]);
-  }
-  __syncthreads();
-  if (tid < nc) {   // rank by counting: flat indices are distinct, so the ranks are a permutation
-    int rank = 0;
-    for (int o = 0; o < nc; ++o) rank += bm_better(m_s[o], m_i[o], m_s[tid], m_i[tid]) ? 1 : 0;
-    if (rank < k2) { t_s[rank] = m_s[tid]; t_i[rank] = m_i[tid]; }
+  if constexpr (SAMPLE) {
+    // the request's 2k draws are its top 2k keys; they are then ranked by warped score (ties to the lower flat index)
+    __shared__ float m_w[BM_MAX_K * 2 * BM_MAX_K];
+    __shared__ float d_w[2 * BM_MAX_K];
+    __shared__ int d_i[2 * BM_MAX_K];
+    for (int c = tid; c < nc; c += BM_THREADS) {
+      const int idx = (r0 + c / k2) * 2 * BM_MAX_K + c % k2;
+      m_s[c] = __ldcg(&cand_s[idx]);
+      m_i[c] = __ldcg(&cand_i[idx]);
+      m_w[c] = __ldcg(&cand_w[idx]);
+    }
+    __syncthreads();
+    if (tid < nc) {
+      int rank = 0;
+      for (int o = 0; o < nc; ++o) rank += bm_better(m_s[o], m_i[o], m_s[tid], m_i[tid]) ? 1 : 0;
+      if (rank < k2) { d_w[rank] = m_w[tid]; d_i[rank] = m_i[tid]; }
+    }
+    __syncthreads();
+    if (tid < k2) {
+      int rank = 0;
+      for (int o = 0; o < k2; ++o) rank += bm_better(d_w[o], d_i[o], d_w[tid], d_i[tid]) ? 1 : 0;
+      t_s[rank] = d_w[tid];
+      t_i[rank] = d_i[tid];
+    }
+  } else {
+    for (int c = tid; c < nc; c += BM_THREADS) {
+      const int idx = (r0 + c / k2) * 2 * BM_MAX_K + c % k2;
+      m_s[c] = __ldcg(&cand_s[idx]);
+      m_i[c] = __ldcg(&cand_i[idx]);
+    }
+    __syncthreads();
+    if (tid < nc) {   // rank by counting: flat indices are distinct, so the ranks are a permutation
+      int rank = 0;
+      for (int o = 0; o < nc; ++o) rank += bm_better(m_s[o], m_i[o], m_s[tid], m_i[tid]) ? 1 : 0;
+      if (rank < k2) { t_s[rank] = m_s[tid]; t_i[rank] = m_i[tid]; }
+    }
   }
   __syncthreads();
 
@@ -968,16 +1111,18 @@ extern "C" int vb200_sample_advance(const float* logits, int64_t ld, int64_t row
 }
 
 extern "C" size_t vb200_beam_workspace_size(int64_t rows) {
-  return BM_COUNTER_BYTES + static_cast<size_t>(rows > 0 ? rows : 0) * 2 * BM_MAX_K * (sizeof(float) + sizeof(int32_t));
+  // [counters | candidate scores | flat indices | warped scores (beam sampling)] x 2 * BM_MAX_K per row
+  return BM_COUNTER_BYTES + static_cast<size_t>(rows > 0 ? rows : 0) * 2 * BM_MAX_K * (2 * sizeof(float) + sizeof(int32_t));
 }
 
-extern "C" int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
-                                  const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
-                                  int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len,
-                                  int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld,
-                                  int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
-                                  int64_t log_stride, const int32_t* prompt_len, void* workspace,
-                                  size_t workspace_bytes, cudaStream_t stream) {
+template <bool SAMPLE>
+static int launch_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                               const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
+                               int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len, int32_t* hyp_seq,
+                               int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld, int32_t* next_src, int32_t* positions,
+                               int32_t* kv_len, int64_t* token_log, int64_t log_stride, const int32_t* prompt_len,
+                               void* workspace, size_t workspace_bytes, const vb_sample_params* sample_params,
+                               cudaStream_t stream) {
   VB_CHECK_ARG(logits && params && beam_score && parent && done && beam_src && hyp_score && hyp_len && hyp_seq &&
                hyp_count && hyp_ids && next_src && positions && kv_len && token_log && prompt_len);
   VB_CHECK_ARG(B > 0 && k > 0 && n >= 2 && ld >= n && src_ld > 0 && src_ld <= INT_MAX && hyp_ld > 0 &&
@@ -988,7 +1133,7 @@ extern "C" int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, in
   if (!workspace || workspace_bytes < vb200_beam_workspace_size(rows)) return VB_ERR_WORKSPACE;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(beam_advance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(beam_advance_kernel<SAMPLE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          BM_MAX_N * static_cast<int>(sizeof(float)));
     if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
     attr_set = true;
@@ -996,14 +1141,41 @@ extern "C" int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, in
   int32_t* counters = reinterpret_cast<int32_t*>(workspace);
   float* cand_s = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + BM_COUNTER_BYTES);
   int32_t* cand_i = reinterpret_cast<int32_t*>(cand_s + rows * 2 * BM_MAX_K);
-  cudaError_t e = vb_launch(beam_advance_kernel, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS),
+  float* cand_w = reinterpret_cast<float*>(cand_i + rows * 2 * BM_MAX_K);
+  cudaError_t e = vb_launch(beam_advance_kernel<SAMPLE>, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS),
                             static_cast<size_t>(n) * sizeof(float), stream, logits, static_cast<long long>(ld),
                             static_cast<int>(n), static_cast<int>(k), params, beam_score, parent, done, beam_src,
                             static_cast<int>(src_ld), hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
                             static_cast<int>(hyp_ld), next_src, positions, kv_len, token_log,
-                            static_cast<int>(log_stride), prompt_len, cand_s, cand_i, counters);
+                            static_cast<int>(log_stride), prompt_len, cand_s, cand_i, counters, sample_params, cand_w);
   if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
   return VB_OK;
+}
+
+extern "C" int vb200_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                  const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
+                                  int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len,
+                                  int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld,
+                                  int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
+                                  int64_t log_stride, const int32_t* prompt_len, void* workspace,
+                                  size_t workspace_bytes, cudaStream_t stream) {
+  return launch_beam_advance<false>(logits, ld, B, k, n, params, beam_score, parent, done, beam_src, src_ld, hyp_score,
+                                    hyp_len, hyp_seq, hyp_count, hyp_ids, hyp_ld, next_src, positions, kv_len,
+                                    token_log, log_stride, prompt_len, workspace, workspace_bytes, nullptr, stream);
+}
+
+extern "C" int vb200_beam_sample_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                         const vb_beam_params* params, float* beam_score, int32_t* parent,
+                                         int32_t* done, int32_t* beam_src, int64_t src_ld, double* hyp_score,
+                                         int32_t* hyp_len, int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids,
+                                         int64_t hyp_ld, int32_t* next_src, int32_t* positions, int32_t* kv_len,
+                                         int64_t* token_log, int64_t log_stride, const int32_t* prompt_len,
+                                         void* workspace, size_t workspace_bytes, const vb_sample_params* sample_params,
+                                         cudaStream_t stream) {
+  VB_CHECK_ARG(sample_params != nullptr);
+  return launch_beam_advance<true>(logits, ld, B, k, n, params, beam_score, parent, done, beam_src, src_ld, hyp_score,
+                                   hyp_len, hyp_seq, hyp_count, hyp_ids, hyp_ld, next_src, positions, kv_len, token_log,
+                                   log_stride, prompt_len, workspace, workspace_bytes, sample_params, stream);
 }
 
 extern "C" int vb200_rope_kv_append(void* qkv, int64_t ld_qkv, const int32_t* positions,

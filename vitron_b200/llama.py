@@ -482,9 +482,9 @@ class LlamaEngine:
             lib.vb200_set_pdl(prev)
 
     def _step_kernels_inner(self, B, sampled=False):
-        if sampled == "beam":
+        if sampled in ("beam", "beam_sample"):
             self._decode_body(B, beam=True)
-            self.beam_advance(self.d_logits[:B])
+            self.beam_advance(self.d_logits[:B], sample=sampled == "beam_sample")
             return
         self._decode_body(B)
         # token_log[b, d_len - d_prompt] = token; d_src = token; d_pos += 1; d_len += 1
@@ -525,47 +525,64 @@ class LlamaEngine:
         if self.beam is None or self.beam_k < 1:
             raise RuntimeError("no beam search is set up on this engine: call start_beam() before beam steps")
 
-    def beam_advance(self, logits):
-        """The beam step over rows of fp32 logits with the start_beam parameters. A CUDA engine runs the kernel; a CPU
-        engine, which runs no kernels of this library, runs the host statement of the same contract (vitron_b200.beam)."""
+    def beam_advance(self, logits, sample=False):
+        """The beam step over rows of fp32 logits with the start_beam parameters (sample=True: the beam-sampling step,
+        with the set_sampling parameters too). A CUDA engine runs the kernel; a CPU engine, which runs no kernels of this
+        library, runs the host statement of the same contract (vitron_b200.beam)."""
         self._require_beam()
         R = logits.shape[0]
-        fn = ops.beam_advance if self.device.type == "cuda" else _beam.beam_advance
-        fn(logits, self.beam_k, self.d_beam, **{n: t[:R] for n, t in self.beam.items()}, next_src=self.d_src[:R],
-           positions=self.d_pos[:R], kv_len=self.d_len[:R], token_log=self.token_log[:R], prompt_len=self.d_prompt[:R])
+        state = dict({n: t[:R] for n, t in self.beam.items()}, next_src=self.d_src[:R], positions=self.d_pos[:R],
+                     kv_len=self.d_len[:R], token_log=self.token_log[:R], prompt_len=self.d_prompt[:R])
+        if sample:
+            fn = ops.beam_sample_advance if self.device.type == "cuda" else _beam.beam_sample_advance
+            fn(logits, self.beam_k, self.d_beam, self.d_sample, **state)
+        else:
+            fn = ops.beam_advance if self.device.type == "cuda" else _beam.beam_advance
+            fn(logits, self.beam_k, self.d_beam, **state)
 
-    def start_beam(self, logits, k, max_new_tokens, params):
+    def start_beam(self, logits, k, max_new_tokens, params, sample=False, searches=1):
         """Beam search over the B prompts of the last prefill: logits [B, V] are its last-token logits, params a
         beam.pack_params buffer. Rows b * k + j become the beams of request b, sharing its full prompt pages (the partial
         last page is copied per beam); step 0 runs the beam kernel on the logits replicated to the k rows (generated
-        token 0). decode_steps(B * k, n, sampled="beam") then runs further steps."""
+        token 0). decode_steps(B * k, n, sampled="beam") then runs further steps.
+
+        sample=True is beam sampling with the set_sampling parameters (decode_steps(..., sampled="beam_sample")), every
+        beam starting at score 0, and
+        searches = r runs r independent searches per prompt: search b * r + i (rows (b * r + i) * k + j) samples prompt
+        b, so the prompt's pages are shared by r * k rows."""
         B = logits.shape[0]
-        R, lens = B * k, [int(x) for x in self._lens_host[:B]]
+        R, lens = B * searches * k, [int(x) for x in self._lens_host[:B]]
         if not 1 <= k <= _beam.MAX_K:
             raise ValueError(f"num_beams must be in 1..{_beam.MAX_K}, got {k}")
+        if searches < 1:
+            raise ValueError(f"searches must be >= 1, got {searches}")
         if R > self.max_batch:
-            raise ValueError(f"batch {B} x num_beams {k} = {R} rows > engine max_batch {self.max_batch}")
+            raise ValueError(f"batch {B} x {searches} searches x num_beams {k} = {R} rows > engine max_batch "
+                             f"{self.max_batch}")
         need = max(lens) + max_new_tokens
         if need > self.cache.max_seq_len:
             raise ValueError(f"prompt + max_new_tokens = {need} exceeds KV capacity {self.cache.max_seq_len}")
         st = self._beam_state()
-        self.cache.fork(lens, k)
+        self.cache.fork(lens, searches * k)
+        rk = searches * k
         for r in range(R):
-            self.cache.reserve(r, lens[r // k] + max_new_tokens)
+            self.cache.reserve(r, lens[r // rk] + max_new_tokens)
         self.cache.sync_table()
         self.beam_k = k
         self.d_beam.copy_(params)
-        plen = torch.tensor(lens, dtype=torch.int32).repeat_interleave(k).to(self.device)
+        plen = torch.tensor(lens, dtype=torch.int32).repeat_interleave(rk).to(self.device)
         self.d_prompt[:R].copy_(plen)
         self.d_len[:R].copy_(plen)            # kv_len - prompt_len = 0: the step below logs generated token 0
         self.d_pos[:R].copy_(plen - 1)
         self._lens_host = plen.tolist()
-        init = torch.full((B, k), -1e9, dtype=torch.float32)
+        init = torch.full((B * searches, k), -1e9, dtype=torch.float32)
         init[:, 0] = 0.0
+        if sample:              # 4.31 beam_sample starts every beam at 0 (beam_search starts beams 1..k-1 at -1e9)
+            init.zero_()
         st["beam_score"][:R].copy_(init.reshape(-1))
         for name in ("done", "hyp_count"):
-            st[name][:B].zero_()
-        self.beam_advance(logits.float().repeat_interleave(k, 0).contiguous())
+            st[name][:B * searches].zero_()
+        self.beam_advance(logits.float().repeat_interleave(rk, 0).contiguous(), sample=sample)
 
     def start_decode(self, first_tokens, max_new_tokens):
         """first_tokens [B] int64: the token chosen from the prefill logits (already counted as
@@ -585,22 +602,24 @@ class LlamaEngine:
 
     def decode_steps(self, B, n, use_graph=True, sampled=False):
         """Run n decode steps for slots 0..B-1 (no host sync): greedy, sampled with the set_sampling parameters, or
-        (sampled="beam") beam steps over the B = requests x num_beams rows of start_beam."""
+        (sampled="beam" / "beam_sample") beam-search / beam-sampling steps over the B = searches x num_beams rows of
+        start_beam. The beam modes read their parameters from device buffers: one graph per (rows, mode, k)."""
         if n <= 0:
             return
-        if sampled == "beam":
+        beam_mode = sampled in ("beam", "beam_sample")
+        if beam_mode:
             self._require_beam()
         if not use_graph or self.device.type != "cuda":   # (host-logic tests drive the same step un-graphed)
             for _ in range(n):
                 self._step_kernels(B, sampled)
             return
-        key = (B, "beam", self.beam_k) if sampled == "beam" else (B, bool(sampled))
+        key = (B, sampled, self.beam_k) if beam_mode else (B, bool(sampled))
         if key not in self._graphs:
             # warm-up on a side stream (allocator + lazy init), then capture
             s = torch.cuda.Stream(device=self.device)
             s.wait_stream(torch.cuda.current_stream())
             state = [self.d_src, self.d_pos, self.d_len, self.token_log]
-            if sampled == "beam":
+            if beam_mode:
                 state += list(self.beam.values())
             saved = [t.clone() for t in state]
             with torch.cuda.stream(s):

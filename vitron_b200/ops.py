@@ -615,10 +615,9 @@ def reserve_beam_workspace(rows, device):
     return workspace(_lib.load().vb200_beam_workspace_size(rows), torch.device(device), "beam")
 
 
-def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
-                 next_src, positions, kv_len, token_log, prompt_len):
-    """One beam-search step for B = rows / k requests (contract in include/vitron_b200.h, statement in
-    vitron_b200.beam): parameters from the device buffer `params` (beam.pack_params), state updated in place."""
+def _beam_args(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
+               next_src, positions, kv_len, token_log, prompt_len):
+    """Checks of the beam-step buffers; returns the leading C arguments and the workspace of vb200_beam_(sample_)advance."""
     lib = _lib.load()
     _req(logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1, "fp32 logits [B * k, V]")
     R = logits.shape[0]
@@ -640,12 +639,34 @@ def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_scor
              f"{name}: contiguous {dt} [>= {R}] on the logits' device")
     need = lib.vb200_beam_workspace_size(R)
     ws = workspace(need, logits.device, "beam")
-    check(lib.vb200_beam_advance(logits.data_ptr(), logits.stride(0), R // k, k, logits.shape[1], params.data_ptr(),
-                                 beam_score.data_ptr(), parent.data_ptr(), done.data_ptr(), beam_src.data_ptr(),
-                                 beam_src.stride(0), hyp_score.data_ptr(), hyp_len.data_ptr(), hyp_seq.data_ptr(),
-                                 hyp_count.data_ptr(), hyp_ids.data_ptr(), hyp_ids.stride(0), next_src.data_ptr(),
-                                 positions.data_ptr(), kv_len.data_ptr(), token_log.data_ptr(), token_log.stride(0),
-                                 prompt_len.data_ptr(), ws.data_ptr(), need, _stream()), "vb200_beam_advance")
+    return (logits.data_ptr(), logits.stride(0), R // k, k, logits.shape[1], params.data_ptr(), beam_score.data_ptr(),
+            parent.data_ptr(), done.data_ptr(), beam_src.data_ptr(), beam_src.stride(0), hyp_score.data_ptr(),
+            hyp_len.data_ptr(), hyp_seq.data_ptr(), hyp_count.data_ptr(), hyp_ids.data_ptr(), hyp_ids.stride(0),
+            next_src.data_ptr(), positions.data_ptr(), kv_len.data_ptr(), token_log.data_ptr(), token_log.stride(0),
+            prompt_len.data_ptr(), ws.data_ptr(), need)
+
+
+def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
+                 next_src, positions, kv_len, token_log, prompt_len):
+    """One beam-search step for B = rows / k requests (contract in include/vitron_b200.h, statement in
+    vitron_b200.beam): parameters from the device buffer `params` (beam.pack_params), state updated in place."""
+    args = _beam_args(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
+                      hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
+    check(_lib.load().vb200_beam_advance(*args, _stream()), "vb200_beam_advance")
+    _launches[0] += 1
+
+
+def beam_sample_advance(logits, k, params, sample_params, beam_score, parent, done, beam_src, hyp_score, hyp_len,
+                        hyp_seq, hyp_count, hyp_ids, next_src, positions, kv_len, token_log, prompt_len):
+    """One beam-sampling step (HF 4.31 beam_sample) for B = rows / k searches: beam_advance's arguments plus the device
+    buffer `sample_params` (sample_params: temperature, top_k, top_p, seed). Contract in include/vitron_b200.h,
+    statement in vitron_b200.beam.beam_sample_advance."""
+    _req(sample_params.dtype == torch.uint8 and sample_params.numel() == SAMPLE_PARAMS.size
+         and sample_params.is_contiguous() and sample_params.device == logits.device,
+         f"sample_params: uint8 [{SAMPLE_PARAMS.size}] sampling buffer on the logits' device")
+    args = _beam_args(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
+                      hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
+    check(_lib.load().vb200_beam_sample_advance(*args, sample_params.data_ptr(), _stream()), "vb200_beam_sample_advance")
     _launches[0] += 1
 
 

@@ -22,9 +22,10 @@ def philox4x32_10(counter, key):
     return np.stack(c, -1)
 
 
-def sample_support(logits, temperature, top_k, top_p):
+def sample_support(logits, temperature, top_k, top_p, min_keep=1):
     """Steps 1-4 of the contract in float64 for logits [B, V]: (kept bool [B, V], p float64 [B, V] zero outside the kept
-    set, near_cut bool [B]: a kept token's top-p fraction lies within 1e-5 of top_p)."""
+    set, near_cut bool [B]: a kept token's top-p fraction lies within 1e-5 of top_p). min_keep = 2 (beam sampling) also
+    keeps, through top-p, every token with fewer than 2 strictly larger z among the tokens top-k kept."""
     l = logits.detach().double().cpu()
     B, V = l.shape
     neg_inf = torch.tensor(float("-inf"), dtype=torch.float64)
@@ -42,6 +43,7 @@ def sample_support(logits, temperature, top_k, top_p):
     p = torch.where(z == zmax, torch.ones_like(z), torch.exp(z - zmax))
     p = torch.where(kept, p, torch.zeros_like(p))
     near = torch.zeros(B, dtype=torch.bool)
+    kept_k = kept.clone()
     if top_p < 1.0:
         if top_p <= 0.0:
             kept &= z == zmax
@@ -55,6 +57,10 @@ def sample_support(logits, temperature, top_k, top_p):
             frac = above / total
             near |= (kept & ((frac - float(top_p)).abs() < 1e-5)).any(1)
             kept &= (frac < float(top_p)) | (z == zmax)
+        if min_keep > 1:
+            zs0 = torch.where(kept_k, z, neg_inf).sort(dim=1, descending=True).values
+            larger = torch.searchsorted(-zs0.contiguous(), -z.contiguous(), right=False)   # kept z strictly above
+            kept |= kept_k & (larger < min_keep)
         p = torch.where(kept, p, torch.zeros_like(p))
     return kept, p, near
 

@@ -508,8 +508,15 @@ class VitronLlamaForCausalLM(ModuleFace):
         as [B * num_return_sequences, input_len + gen_len]. The prompt (and its images) is prefilled once per request;
         its beams share its KV pages, and the beam step runs on the device inside the graphed decode step, so the host
         reads the done flags once per `sync_every` steps. With stopping_criteria the running beams are rebuilt after
-        every step (beams reorder their history), which syncs once per step. do_sample=True ignores num_beams, as
-        before: beam sampling is not implemented."""
+        every step (beams reorder their history), which syncs once per step.
+
+        do_sample=True with num_beams > 1 is HF 4.31 beam sampling (`beam_sample`), stated in vitron_b200.beam: the
+        warpers (temperature, top_k at least 2, top_p keeping at least 2) apply to the running scores, 2 * num_beams
+        candidates per search are drawn without replacement on the device, and the scorer is beam search's.
+        num_return_sequences = r runs r independent searches per request and returns each one's best hypothesis:
+        [B * r, input_len + gen_len], request-major; B * r * num_beams rows must fit the engine's max_batch. The seed is
+        drawn from torch's default CPU generator as in sampling; prefill, page sharing, sync_every and
+        stopping_criteria behave as in beam search."""
         if input_ids is None:
             input_ids = inputs
         eos = self.config.eos_token_id if eos_token_id is None else eos_token_id
@@ -517,6 +524,7 @@ class VitronLlamaForCausalLM(ModuleFace):
         eos_set = set(eos if isinstance(eos, (list, tuple)) else [eos]) if eos is not None else set()
         B = input_ids.shape[0]
         beam_search = num_beams > 1 and not do_sample
+        beam_sample = num_beams > 1 and do_sample
         if beam_search:
             if num_return_sequences > num_beams:
                 raise ValueError(f"num_return_sequences ({num_return_sequences}) has to be smaller or equal to "
@@ -524,6 +532,9 @@ class VitronLlamaForCausalLM(ModuleFace):
             if B * num_beams > self.engine.max_batch:
                 raise ValueError(f"batch {B} x num_beams {num_beams} = {B * num_beams} rows > engine max_batch "
                                  f"{self.engine.max_batch}")
+        if beam_sample and B * num_return_sequences * num_beams > self.engine.max_batch:
+            raise ValueError(f"batch {B} x num_return_sequences {num_return_sequences} x num_beams {num_beams} = "
+                             f"{B * num_return_sequences * num_beams} rows > engine max_batch {self.engine.max_batch}")
         self._kv_segments = None          # the prefill and decode below overwrite the cache: every handle becomes stale
         if images is not None:
             _, _, am, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(
@@ -535,13 +546,14 @@ class VitronLlamaForCausalLM(ModuleFace):
         embeds, lens, _ = self._right_pad(embeds, am)
         eng = self.engine
         logits = eng.prefill(embeds, lens)
-        if beam_search:
-            eos_list = sorted(eos_set) if not isinstance(eos, (list, tuple)) else [int(e) for e in eos]
-            return self._beam_search(input_ids, logits, num_beams, num_return_sequences, length_penalty, early_stopping,
-                                     eos_list, pad, max_new_tokens, stopping_criteria, sync_every)
         if do_sample:
             seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64)) & (2 ** 64 - 1)
             eng.set_sampling(temperature, top_k, top_p, seed)
+        if beam_search or beam_sample:
+            eos_list = sorted(eos_set) if not isinstance(eos, (list, tuple)) else [int(e) for e in eos]
+            return self._beam_search(input_ids, logits, num_beams, num_return_sequences, length_penalty, early_stopping,
+                                     eos_list, pad, max_new_tokens, stopping_criteria, sync_every, sample=beam_sample)
+        if do_sample:
             first = eng.sample_advance(logits)                        # generated token 0: Philox step 0
         else:
             first = ops.argmax_rows(logits)
@@ -577,27 +589,32 @@ class VitronLlamaForCausalLM(ModuleFace):
         return torch.cat([input_ids, gen.to(input_ids.device)], 1)
 
     def _beam_search(self, input_ids, logits, k, nrs, length_penalty, early_stopping, eos, pad, max_new_tokens,
-                     stopping_criteria, sync_every):
+                     stopping_criteria, sync_every, sample=False):
         eng = self.engine
-        B, n_in = input_ids.shape
+        n_in = input_ids.shape[1]
+        # beam sampling runs nrs searches per request and keeps the best of each; beam search keeps nrs of one search
+        searches, keep = (nrs, 1) if sample else (1, nrs)
+        prompts = input_ids.repeat_interleave(searches, 0)   # the prompt of each search
+        B = prompts.shape[0]
         R = B * k
         if pad is None:
             pad = eos[0] if eos else 0
         prm = dict(length_penalty=float(length_penalty), early_stopping=early_stopping, pad=int(pad), input_len=n_in,
                    max_length=n_in + max_new_tokens, eos=eos)
         eng.start_beam(logits, k, max_new_tokens, beam.pack_params(length_penalty, early_stopping, pad, n_in,
-                                                                   n_in + max_new_tokens, eos))
+                                                                   n_in + max_new_tokens, eos),
+                       sample=sample, searches=searches)
         st = eng.beam
         produced = 1
         while produced < max_new_tokens:
             if bool(st["done"][:B].cpu().all()):
                 break
             if stopping_criteria is not None:
-                seq = torch.cat([input_ids.cpu().repeat_interleave(k, 0), self._running(produced, R)], 1)
+                seq = torch.cat([prompts.cpu().repeat_interleave(k, 0), self._running(produced, R)], 1)
                 if self._criteria_met(stopping_criteria, seq.to(input_ids.device)):
                     break
             n = 1 if stopping_criteria is not None else min(sync_every, max_new_tokens - produced)
-            eng.decode_steps(R, n, sampled="beam")
+            eng.decode_steps(R, n, sampled="beam_sample" if sample else "beam")
             produced += n
         done = st["done"][:B].cpu().tolist()
         hs, hl, hq = st["hyp_score"][:R].cpu(), st["hyp_len"][:R].cpu(), st["hyp_seq"][:R].cpu()
@@ -608,8 +625,8 @@ class VitronLlamaForCausalLM(ModuleFace):
             h.slots = [dict(score=float(hs[b * k + s]), length=int(hl[b * k + s]), seq=int(hq[b * k + s]),
                             ids=ids[b * k + s, :int(hl[b * k + s]) - n_in]) for s in range(counts[b])]
             hyps.append(h)
-        gen = beam.finalize(hyps, done, st["beam_score"][:R].cpu(), self._running(produced, R), nrs, prm)
-        return torch.cat([input_ids.repeat_interleave(nrs, 0), gen.to(input_ids.device)], 1)
+        gen = beam.finalize(hyps, done, st["beam_score"][:R].cpu(), self._running(produced, R), keep, prm)
+        return torch.cat([prompts.repeat_interleave(keep, 0), gen.to(input_ids.device)], 1)
 
     def _running(self, t, R):
         eng = self.engine
