@@ -353,6 +353,55 @@ int vb200_beam_sample_advance(const float* logits, int64_t ld, int64_t B, int64_
                               int32_t* positions, int32_t* kv_len, int64_t* token_log, int64_t log_stride,
                               const int32_t* prompt_len, void* workspace, size_t workspace_bytes,
                               const vb_sample_params* sample_params, cudaStream_t stream);
+/* vb200_beam_advance / vb200_beam_sample_advance over rows that already hold (processed) log-probabilities, as
+ * vb200_logits_process(logprobs = 1) writes them: the candidate score is logits[r, i] + beam_score[r] (no log-softmax
+ * of its own); the warpers of beam sampling cut on (logits[r, i] - max_i logits[r, i]) / T, which is what they cut on
+ * without processors. Arguments, limits and bookkeeping as the two entries above. */
+int vb200_beam_advance_logprobs(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
+                                int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len, int32_t* hyp_seq,
+                                int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld, int32_t* next_src,
+                                int32_t* positions, int32_t* kv_len, int64_t* token_log, int64_t log_stride,
+                                const int32_t* prompt_len, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int vb200_beam_sample_advance_logprobs(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                       const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
+                                       int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len,
+                                       int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids, int64_t hyp_ld,
+                                       int32_t* next_src, int32_t* positions, int32_t* kv_len, int64_t* token_log,
+                                       int64_t log_stride, const int32_t* prompt_len, void* workspace,
+                                       size_t workspace_bytes, const vb_sample_params* sample_params,
+                                       cudaStream_t stream);
+
+/* Logits-processor parameters, read by the kernel from DEVICE memory (one captured decode graph serves every setting). */
+typedef struct vb_proc_params {
+  float repetition_penalty;      /* 1 = off; > 0 */
+  int32_t no_repeat_ngram_size;  /* 0 = off */
+  int32_t min_length;            /* 0 = off */
+  int32_t min_new_tokens;        /* 0 = off */
+  int32_t input_len;             /* input_ids.shape[1]: prompt columns of every row, sentinels and left padding included */
+  int32_t n_eos;                 /* 0..8 */
+  int32_t eos[8];
+} vb_proc_params;                /* 56 bytes */
+
+/* HF 4.31 logits processors, in place on rows of fp32 scores, in the order 4.31's _get_logits_processor applies them;
+ * stated in fp32 in vitron_b200/processors.py. Row r's history (4.31's input_ids row) is prompt_ids[r, 0:input_len]
+ * (int32, row stride prompt_ld >= input_len) followed by its t = kv_len[r] - prompt_len[r] generated ids: id j is
+ * token_log[s, j], s = beam_src[r, prompt_len[r] + j] for beam rows, else s = r. Without kv_len / prompt_len, t = 0 (the
+ * prefill logits; token_log and beam_src are not read). cur_len = input_len + t.
+ *   logprobs = 1: the row is first replaced by its log-softmax (NaN counts as -inf), computed as vb200_beam_advance
+ *     does, bit for bit (the scores 4.31's beam search processes);
+ *   repetition_penalty p != 1: every distinct id of the history in [0, n) once: s = s < 0 ? s * p : s / p (fp32,
+ *     correctly rounded); sentinel ids (< 0) are skipped;
+ *   no_repeat_ngram_size g > 0: if cur_len + 1 >= g, every id that followed an earlier occurrence of the last g - 1
+ *     history ids becomes -inf (g = 1: every history id); sentinels match like any id but are never banned;
+ *   min_length > 0 and cur_len < min_length, or min_new_tokens > 0 and t < min_new_tokens: every eos id in [0, n)
+ *     becomes -inf.
+ * One CTA per row; n <= 49152 and prompt_ld (+ log_stride when kv_len is given) <= 8192 staged history tokens, else
+ * VB_ERR_UNSUPPORTED. The result does not depend on thread order. */
+int vb200_logits_process(float* logits, int64_t ld, int64_t rows, int64_t n, const vb_proc_params* params,
+                         const int32_t* prompt_ids, int64_t prompt_ld, const int64_t* token_log, int64_t log_stride,
+                         const int32_t* beam_src, int64_t src_ld, const int32_t* kv_len, const int32_t* prompt_len,
+                         int logprobs, cudaStream_t stream);
 
 /* ---- vision / diffusion glue (vision.cu) ----------------------------------------------------
  * patchify: NCHW pixels -> [nb*gh*gw, kpad] rows ordered (c, py, px) for the patch-embed GEMM

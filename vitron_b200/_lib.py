@@ -78,6 +78,11 @@ SIGNATURES = {
                                   _p, _p, _i64, _p, _p, _sz, _p]),
     "vb200_beam_sample_advance": (_i32, [_p, _i64, _i64, _i64, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64,
                                          _p, _p, _p, _p, _i64, _p, _p, _sz, _p, _p]),
+    "vb200_beam_advance_logprobs": (_i32, [_p, _i64, _i64, _i64, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64,
+                                           _p, _p, _p, _p, _i64, _p, _p, _sz, _p]),
+    "vb200_beam_sample_advance_logprobs": (_i32, [_p, _i64, _i64, _i64, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p,
+                                                  _i64, _p, _p, _p, _p, _i64, _p, _p, _sz, _p, _p]),
+    "vb200_logits_process": (_i32, [_p, _i64, _i64, _i64, _p, _p, _i64, _p, _i64, _p, _i64, _p, _p, _i32, _p]),
     "vb200_patchify": (_i32, [_p, _i32, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p]),
     "vb200_vit_embed_ln": (_i32, [_p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _f, _p]),
     "vb200_upsample2x_nhwc": (_i32, [_p, _p, _i64, _i64, _i64, _i64, _p]),

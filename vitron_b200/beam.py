@@ -165,9 +165,10 @@ def process(cands, k, V, hyps, t, prm):
 
 
 def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
-                 next_src, positions, kv_len, token_log, prompt_len):
-    """Same arguments and bookkeeping as ops.beam_advance, on host tensors."""
-    lsm = log_softmax64(logits)
+                 next_src, positions, kv_len, token_log, prompt_len, logprobs=False):
+    """Same arguments and bookkeeping as ops.beam_advance, on host tensors. logprobs=True: the rows already hold
+    (processed) log-probabilities, vitron_b200.processors' logprobs output."""
+    lsm = _logprobs(logits) if logprobs else log_softmax64(logits)
 
     def cands(b, r0, t):
         return top_candidates(lsm[r0:r0 + k] + beam_score[r0:r0 + k].double().cpu()[:, None], k)
@@ -175,10 +176,17 @@ def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_scor
              hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
 
 
-def warped_scores(logits, beam_score, temperature):
+def _logprobs(rows):
+    """Rows that already hold log-probabilities, as float64 (NaN as -inf)."""
+    l = rows.detach().cpu().float().double()
+    return torch.where(torch.isnan(l), torch.full_like(l, float("-inf")), l)
+
+
+def warped_scores(logits, beam_score, temperature, logprobs=False):
     """Rule 2s up to the cuts: w = (log_softmax(logits) + beam_score) / T, float64 [R, V]; a w that fp32 cannot hold is
-    -inf."""
-    w = (log_softmax64(logits) + beam_score.double().cpu()[:, None]) / float(temperature)
+    -inf. logprobs=True: the rows are log-probabilities already."""
+    lsm = _logprobs(logits) if logprobs else log_softmax64(logits)
+    w = (lsm + beam_score.double().cpu()[:, None]) / float(temperature)
     return torch.where(torch.isinf(w.float()), torch.full_like(w, float("-inf")), w)
 
 
@@ -217,11 +225,11 @@ def sample_draws(w, kept, k, b, t, seed):
 
 
 def beam_sample_advance(logits, k, params, sample_params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq,
-                        hyp_count, hyp_ids, next_src, positions, kv_len, token_log, prompt_len):
-    """Same arguments and bookkeeping as ops.beam_sample_advance, on host tensors."""
+                        hyp_count, hyp_ids, next_src, positions, kv_len, token_log, prompt_len, logprobs=False):
+    """Same arguments and bookkeeping as ops.beam_sample_advance, on host tensors (logprobs as in beam_advance)."""
     from .ops import SAMPLE_PARAMS
     temperature, top_k, top_p, _, seed = SAMPLE_PARAMS.unpack(sample_params.cpu().numpy().tobytes())
-    w = warped_scores(logits, beam_score, temperature)
+    w = warped_scores(logits, beam_score, temperature, logprobs)
     kept, _ = warp_kept(w, top_k, top_p)
 
     def cands(b, r0, t):

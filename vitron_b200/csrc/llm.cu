@@ -764,6 +764,33 @@ struct BmStage<true> {
   __device__ static int32_t (&get(type& s))[BM_MAX_K][BM_STAGE] { return s.stage; }
 };
 
+// The block-wide max and sum of the row log-softmax (BM_THREADS threads, s_f: 32 floats). The beam kernel and the logits
+// processors' LOGPROBS mode share them, so that the log-probabilities the processors write are bit-identical to the ones
+// the beam kernel computes itself.
+__device__ __forceinline__ float bm_block_max(float mx, float* s_f, int lane, int warp) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane == 0) s_f[warp] = mx;
+  __syncthreads();
+  mx = s_f[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  __syncthreads();
+  return mx;
+}
+
+__device__ __forceinline__ float bm_block_sum(float sum, float* s_f, int lane, int warp) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  if (lane == 0) s_f[warp] = sum;
+  __syncthreads();
+  sum = s_f[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  __syncthreads();
+  return sum;
+}
+
 // Gumbel noise of flat index f of search b at step t: U = (2 * (x >> 9) + 1) * 2^-24 in (0, 1), x = word f % 4 of
 // Philox4x32-10(counter (t, b, f / 4, 1), key (seed_lo, seed_hi)); the noise is -log(-log U).
 __device__ __forceinline__ float bm_gumbel(uint32_t x) {
@@ -774,7 +801,9 @@ __device__ __forceinline__ float bm_gumbel(uint32_t x) {
 // SAMPLE = false: beam search. SAMPLE = true: beam sampling (HF 4.31 beam_sample): the rows' scores are warped
 // (temperature, top-k, top-p with 2 kept) and 2k candidates per request are drawn without replacement as the top 2k of
 // key = w + Gumbel noise; they are then ranked by warped score and go through the same scorer.
-template <bool SAMPLE>
+// LOGPROBS: the rows already hold (processed) log-probabilities, written by logits_process_kernel's LOGPROBS mode: the
+// candidate score is row[i] + beam score, with no max / sum pass of its own (the warpers still cut on the row's max).
+template <bool SAMPLE, bool LOGPROBS = false>
 __global__ void __launch_bounds__(BM_THREADS, 1)
 beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k, const vb_beam_params* __restrict__ prm,
                     float* __restrict__ beam_score, int32_t* __restrict__ parent, int32_t* __restrict__ done,
@@ -812,29 +841,25 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
     srow[i] = v;
     mx = fmaxf(mx, v);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  if (lane == 0) s_f[warp] = mx;
-  __syncthreads();
-  mx = s_f[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  __syncthreads();
-  float sum = 0.f;
-  if (mx > -INFINITY)
-    for (int i = tid; i < n; i += BM_THREADS) sum += expf(srow[i] - mx);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if (lane == 0) s_f[warp] = sum;
-  __syncthreads();
-  sum = s_f[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  __syncthreads();
-  const float logz = logf(sum);
+  mx = bm_block_max(mx, s_f, lane, warp);
+  float logz = 0.f;
+  if constexpr (!LOGPROBS) {
+    float sum = 0.f;
+    if (mx > -INFINITY)
+      for (int i = tid; i < n; i += BM_THREADS) sum += expf(srow[i] - mx);
+    logz = logf(bm_block_sum(sum, s_f, lane, warp));
+  }
   const float bsc = beam_score[r];
   // candidate score = log_softmax + beam score, as torch computes it: (x - max) - log(sum exp(x - max))
-  auto score_of = [&](int i) -> float { return mx == -INFINITY ? -INFINITY : ((srow[i] - mx) - logz) + bsc; };
+  auto score_of = [&](int i) -> float {
+    if constexpr (LOGPROBS) return mx == -INFINITY ? -INFINITY : srow[i] + bsc;
+    else return mx == -INFINITY ? -INFINITY : ((srow[i] - mx) - logz) + bsc;
+  };
+  // the row's log-probability from its logit as read from memory (warped scores are recomputed from it)
+  auto lp_of = [&](int i) -> float {
+    if constexpr (LOGPROBS) return row[i];
+    else return (row[i] - mx) - logz;
+  };
   float temp = 1.f;
   if constexpr (SAMPLE) {
     // ---- the warpers' kept set, cut on d = (x - max x) / T: within the row the warped scores w are d plus a constant,
@@ -867,7 +892,7 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
         const int i = static_cast<int>(4 * g + q - f0);
         if (4 * g + q < f0 || i >= n) continue;
         const bool keep = order_key(srow[i]) >= thr;
-        const float w = ((((row[i] - mx) - logz) + bsc) / temp);   // the candidate score below, computed the same way
+        const float w = ((lp_of(i) + bsc) / temp);   // the candidate score below, computed the same way
         srow[i] = (keep && w > -INFINITY) ? w + bm_gumbel(xw[q]) : -INFINITY;
       }
     }
@@ -920,7 +945,7 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
                                 // its logit exactly as it was staged
         const bool none = wi == INT_MAX || ws == -INFINITY;
         cand_i[r * 2 * BM_MAX_K + q] = none ? BM_SENTINEL + r * 2 * BM_MAX_K + q : j * n + wi;
-        cand_w[r * 2 * BM_MAX_K + q] = none ? -INFINITY : ((((row[wi] - mx) - logz) + bsc) / temp);
+        cand_w[r * 2 * BM_MAX_K + q] = none ? -INFINITY : ((lp_of(wi) + bsc) / temp);
       } else {
         cand_i[r * 2 * BM_MAX_K + q] = wi == INT_MAX ? BM_SENTINEL + r * 2 * BM_MAX_K + q : j * n + wi;
       }
@@ -1072,6 +1097,111 @@ beam_advance_kernel(const float* __restrict__ logits, long long ld, int n, int k
   if (tid == 0) counters[b] = 0;
 }
 
+// ------------------------------------------------------------------ logits processors (HF 4.31 repetition penalty,
+// no-repeat n-grams, min_length, min_new_tokens), in place on rows of fp32 scores. One CTA per row. The row's history
+// (its raw prompt ids, then its generated ids, read through beam_src for beam rows) is staged in shared memory; every
+// write of a pass goes to a distinct entry or writes the same -inf, and the passes are separated by barriers, so the
+// result does not depend on thread order.
+constexpr int LP_MAX_N = 49152;
+constexpr int LP_MAX_HIST = 8192;   // staged history tokens per row (32 KB)
+
+template <bool LOGPROBS>
+__global__ void __launch_bounds__(BM_THREADS, 1)
+logits_process_kernel(float* __restrict__ logits, long long ld, int n, const vb_proc_params* __restrict__ prm,
+                      const int32_t* __restrict__ prompt_ids, int prompt_ld, const int64_t* __restrict__ token_log,
+                      int log_stride, const int32_t* __restrict__ beam_src, int src_ld,
+                      const int32_t* __restrict__ kv_len, const int32_t* __restrict__ prompt_len) {
+  __shared__ int32_t hist[LP_MAX_HIST];
+  __shared__ uint32_t seen[LP_MAX_N / 32];
+  __shared__ float s_f[32];
+  const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  pdl_wait();      // the logits and the decode state come from the predecessors
+  pdl_trigger();
+  float* row = logits + r * ld;
+  if constexpr (LOGPROBS) {
+    // the beam kernel's log-softmax, in its reduction order: (x - max) - log(sum exp(x - max)), NaN as -inf
+    float mx = -INFINITY;
+    for (int i = tid; i < n; i += BM_THREADS) {
+      float v = row[i];
+      if (v != v) v = -INFINITY;
+      mx = fmaxf(mx, v);
+    }
+    mx = bm_block_max(mx, s_f, lane, warp);
+    float sum = 0.f;
+    if (mx > -INFINITY)
+      for (int i = tid; i < n; i += BM_THREADS) {
+        float v = row[i];
+        if (v != v) v = -INFINITY;
+        sum += expf(v - mx);
+      }
+    const float logz = logf(bm_block_sum(sum, s_f, lane, warp));
+    for (int i = tid; i < n; i += BM_THREADS) {
+      float v = row[i];
+      if (v != v) v = -INFINITY;
+      row[i] = mx == -INFINITY ? -INFINITY : (v - mx) - logz;
+    }
+    __syncthreads();
+  }
+  const float penalty = prm->repetition_penalty;
+  const int ngram = prm->no_repeat_ngram_size;
+  const bool counted = kv_len != nullptr && prompt_len != nullptr;
+  const int t = counted ? min(max(kv_len[r] - prompt_len[r], 0), log_stride) : 0;   // generated tokens so far
+  const int P = counted ? prompt_len[r] : 0;
+  const int in_len = min(max(prm->input_len, 0), prompt_ld);
+  const int L = in_len + t;                       // cur_len = input_ids.shape[-1]; <= LP_MAX_HIST (checked at launch)
+  const int words = (n + 31) >> 5;
+  if (penalty != 1.f || ngram > 0) {
+    for (int j = tid; j < L; j += BM_THREADS) {
+      int32_t tok;
+      if (j < in_len) {
+        tok = prompt_ids[static_cast<long long>(r) * prompt_ld + j];
+      } else {
+        const int g = j - in_len;
+        const int src = (beam_src != nullptr && P + g < src_ld) ? beam_src[static_cast<long long>(r) * src_ld + P + g] : r;
+        tok = static_cast<int32_t>(token_log[static_cast<long long>(src) * log_stride + g]);
+      }
+      hist[j] = tok;
+    }
+    for (int w = tid; w < words; w += BM_THREADS) seen[w] = 0u;
+    __syncthreads();
+    if (penalty != 1.f) {
+      // mark each in-vocabulary id once (sentinels < 0 are skipped), then penalise every marked entry once
+      for (int j = tid; j < L; j += BM_THREADS) {
+        const int tok = hist[j];
+        if (tok >= 0 && tok < n) atomicOr(&seen[tok >> 5], 1u << (tok & 31));
+      }
+      __syncthreads();
+      for (int w = tid; w < words; w += BM_THREADS) {
+        uint32_t bits = seen[w];
+        while (bits) {
+          const int i = (w << 5) + __ffs(bits) - 1;
+          bits &= bits - 1u;
+          const float s = row[i];
+          row[i] = s < 0.f ? __fmul_rn(s, penalty) : __fdiv_rn(s, penalty);
+        }
+      }
+      __syncthreads();
+    }
+    if (ngram > 0 && L + 1 >= ngram) {
+      // window s (0 <= s <= L - ngram) whose first ngram - 1 tokens equal the last ngram - 1 bans its last token
+      const int tail = L - ngram + 1;
+      for (int s = tid; s <= L - ngram; s += BM_THREADS) {
+        bool match = true;
+        for (int q = 0; q < ngram - 1 && match; ++q) match = hist[s + q] == hist[tail + q];
+        const int tok = hist[s + ngram - 1];
+        if (match && tok >= 0 && tok < n) row[tok] = -INFINITY;
+      }
+    }
+  }
+  if (tid == 0 && ((prm->min_length > 0 && L < prm->min_length) || (prm->min_new_tokens > 0 && t < prm->min_new_tokens))) {
+    const int n_eos = min(max(prm->n_eos, 0), 8);
+    for (int e = 0; e < n_eos; ++e) {
+      const int tok = prm->eos[e];
+      if (tok >= 0 && tok < n) row[tok] = -INFINITY;
+    }
+  }
+}
+
 }  // namespace vb
 
 using namespace vb;
@@ -1116,7 +1246,7 @@ extern "C" size_t vb200_beam_workspace_size(int64_t rows) {
   return BM_COUNTER_BYTES + static_cast<size_t>(rows > 0 ? rows : 0) * 2 * BM_MAX_K * (2 * sizeof(float) + sizeof(int32_t));
 }
 
-template <bool SAMPLE>
+template <bool SAMPLE, bool LOGPROBS = false>
 static int launch_beam_advance(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
                                const vb_beam_params* params, float* beam_score, int32_t* parent, int32_t* done,
                                int32_t* beam_src, int64_t src_ld, double* hyp_score, int32_t* hyp_len, int32_t* hyp_seq,
@@ -1134,7 +1264,7 @@ static int launch_beam_advance(const float* logits, int64_t ld, int64_t B, int64
   if (!workspace || workspace_bytes < vb200_beam_workspace_size(rows)) return VB_ERR_WORKSPACE;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(beam_advance_kernel<SAMPLE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(beam_advance_kernel<SAMPLE, LOGPROBS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          BM_MAX_N * static_cast<int>(sizeof(float)));
     if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
     attr_set = true;
@@ -1143,7 +1273,7 @@ static int launch_beam_advance(const float* logits, int64_t ld, int64_t B, int64
   float* cand_s = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + BM_COUNTER_BYTES);
   int32_t* cand_i = reinterpret_cast<int32_t*>(cand_s + rows * 2 * BM_MAX_K);
   float* cand_w = reinterpret_cast<float*>(cand_i + rows * 2 * BM_MAX_K);
-  cudaError_t e = vb_launch(beam_advance_kernel<SAMPLE>, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS),
+  cudaError_t e = vb_launch(beam_advance_kernel<SAMPLE, LOGPROBS>, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS),
                             static_cast<size_t>(n) * sizeof(float), stream, logits, static_cast<long long>(ld),
                             static_cast<int>(n), static_cast<int>(k), params, beam_score, parent, done, beam_src,
                             static_cast<int>(src_ld), hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
@@ -1177,6 +1307,58 @@ extern "C" int vb200_beam_sample_advance(const float* logits, int64_t ld, int64_
   return launch_beam_advance<true>(logits, ld, B, k, n, params, beam_score, parent, done, beam_src, src_ld, hyp_score,
                                    hyp_len, hyp_seq, hyp_count, hyp_ids, hyp_ld, next_src, positions, kv_len, token_log,
                                    log_stride, prompt_len, workspace, workspace_bytes, sample_params, stream);
+}
+
+extern "C" int vb200_beam_advance_logprobs(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                           const vb_beam_params* params, float* beam_score, int32_t* parent,
+                                           int32_t* done, int32_t* beam_src, int64_t src_ld, double* hyp_score,
+                                           int32_t* hyp_len, int32_t* hyp_seq, int32_t* hyp_count, int64_t* hyp_ids,
+                                           int64_t hyp_ld, int32_t* next_src, int32_t* positions, int32_t* kv_len,
+                                           int64_t* token_log, int64_t log_stride, const int32_t* prompt_len,
+                                           void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  return launch_beam_advance<false, true>(logits, ld, B, k, n, params, beam_score, parent, done, beam_src, src_ld,
+                                          hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids, hyp_ld, next_src, positions,
+                                          kv_len, token_log, log_stride, prompt_len, workspace, workspace_bytes, nullptr,
+                                          stream);
+}
+
+extern "C" int vb200_beam_sample_advance_logprobs(const float* logits, int64_t ld, int64_t B, int64_t k, int64_t n,
+                                                  const vb_beam_params* params, float* beam_score, int32_t* parent,
+                                                  int32_t* done, int32_t* beam_src, int64_t src_ld, double* hyp_score,
+                                                  int32_t* hyp_len, int32_t* hyp_seq, int32_t* hyp_count,
+                                                  int64_t* hyp_ids, int64_t hyp_ld, int32_t* next_src,
+                                                  int32_t* positions, int32_t* kv_len, int64_t* token_log,
+                                                  int64_t log_stride, const int32_t* prompt_len, void* workspace,
+                                                  size_t workspace_bytes, const vb_sample_params* sample_params,
+                                                  cudaStream_t stream) {
+  VB_CHECK_ARG(sample_params != nullptr);
+  return launch_beam_advance<true, true>(logits, ld, B, k, n, params, beam_score, parent, done, beam_src, src_ld,
+                                         hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids, hyp_ld, next_src, positions,
+                                         kv_len, token_log, log_stride, prompt_len, workspace, workspace_bytes,
+                                         sample_params, stream);
+}
+
+extern "C" int vb200_logits_process(float* logits, int64_t ld, int64_t rows, int64_t n, const vb_proc_params* params,
+                                    const int32_t* prompt_ids, int64_t prompt_ld, const int64_t* token_log,
+                                    int64_t log_stride, const int32_t* beam_src, int64_t src_ld, const int32_t* kv_len,
+                                    const int32_t* prompt_len, int logprobs, cudaStream_t stream) {
+  VB_CHECK_ARG(logits && params && prompt_ids && rows > 0 && rows <= INT_MAX && n > 0 && ld >= n && prompt_ld > 0 &&
+               prompt_ld <= INT_MAX);
+  VB_CHECK_ARG((kv_len == nullptr) == (prompt_len == nullptr));
+  VB_CHECK_ARG(kv_len == nullptr || (token_log != nullptr && log_stride > 0 && log_stride <= INT_MAX));
+  VB_CHECK_ARG(beam_src == nullptr || (kv_len != nullptr && src_ld > 0 && src_ld <= INT_MAX));
+  if (n > LP_MAX_N || prompt_ld + (kv_len != nullptr ? log_stride : 0) > LP_MAX_HIST) return VB_ERR_UNSUPPORTED;
+  const int ls = kv_len != nullptr ? static_cast<int>(log_stride) : 0;
+  const int sl = beam_src != nullptr ? static_cast<int>(src_ld) : 0;
+  cudaError_t e = logprobs
+      ? vb_launch(logits_process_kernel<true>, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS), 0, stream, logits,
+                  static_cast<long long>(ld), static_cast<int>(n), params, prompt_ids, static_cast<int>(prompt_ld),
+                  token_log, ls, beam_src, sl, kv_len, prompt_len)
+      : vb_launch(logits_process_kernel<false>, dim3(static_cast<unsigned>(rows)), dim3(BM_THREADS), 0, stream, logits,
+                  static_cast<long long>(ld), static_cast<int>(n), params, prompt_ids, static_cast<int>(prompt_ld),
+                  token_log, ls, beam_src, sl, kv_len, prompt_len);
+  if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
+  return VB_OK;
 }
 
 extern "C" int vb200_rope_kv_append(void* qkv, int64_t ld_qkv, const int32_t* positions,

@@ -18,7 +18,7 @@ import torch
 
 from . import nf4 as _nf4
 from . import beam as _beam
-from . import ops, sampling
+from . import ops, processors, sampling
 
 BF16 = torch.bfloat16
 
@@ -168,6 +168,11 @@ class LlamaEngine:
         self.token_log = torch.zeros((B, self.cache.max_seq_len), dtype=torch.int64, device=dev)
         # vb_sample_params read by the sampled step: one captured graph serves every temperature / top-k / top-p / seed
         self.d_sample = torch.zeros((ops.SAMPLE_PARAMS.size,), dtype=torch.uint8, device=dev)
+        # logits processors (set_processors): vb_proc_params and every row's raw prompt ids, read by the step's
+        # logits_process kernel; proc_on selects the graphs that run it
+        self.d_proc = torch.zeros((processors.PARAMS.size,), dtype=torch.uint8, device=dev)
+        self.d_proc_prompt = torch.zeros((B, self.cache.max_seq_len), dtype=torch.int32, device=dev)
+        self.proc_on = False
         self.beam = None       # beam-search state (start_beam), allocated on first use
         self.beam_k = 0        # beams per request of the current beam search; 0 = no beam search started
         self._graphs = {}
@@ -484,9 +489,13 @@ class LlamaEngine:
     def _step_kernels_inner(self, B, sampled=False):
         if sampled in ("beam", "beam_sample"):
             self._decode_body(B, beam=True)
-            self.beam_advance(self.d_logits[:B], sample=sampled == "beam_sample")
+            if self.proc_on:
+                self.process_logits(self.d_logits[:B], step=True, beam=True)
+            self.beam_advance(self.d_logits[:B], sample=sampled == "beam_sample", logprobs=self.proc_on)
             return
         self._decode_body(B)
+        if self.proc_on:
+            self.process_logits(self.d_logits[:B], step=True)
         # token_log[b, d_len - d_prompt] = token; d_src = token; d_pos += 1; d_len += 1
         state = dict(next_src=self.d_src[:B], positions=self.d_pos[:B], kv_len=self.d_len[:B], token_log=self.token_log[:B],
                      prompt_len=self.d_prompt[:B])
@@ -509,6 +518,45 @@ class LlamaEngine:
         p = 1.0 if top_p is None else float(top_p)
         self.d_sample.copy_(ops.sample_params(max(float(temperature), 1e-6), k, p, seed))
 
+    def set_processors(self, prompt_ids, repetition_penalty=1.0, no_repeat_ngram_size=0, min_length=0, min_new_tokens=0,
+                       eos_ids=()):
+        """Turn on the HF 4.31 logits processors (vitron_b200.processors) for the next decode: prompt_ids [R, input_len]
+        are the raw input_ids of engine rows 0..R-1 (a beam row gets its request's row), eos_ids the EOS ids the
+        minimum-length rules ban. The settings follow 4.31's enable rules; with none enabled the processors are off.
+        The step reads them from device buffers, so new settings replay the captured graphs."""
+        settings, on = processors.check_settings(repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens,
+                                                 list(eos_ids))
+        if not on:
+            return self.clear_processors()
+        R, n_in = prompt_ids.shape
+        S = self.cache.max_seq_len
+        if R > self.max_batch:
+            raise ValueError(f"{R} prompt rows > engine max_batch {self.max_batch}")
+        if n_in > S or 2 * S > processors.MAX_HIST:
+            raise ValueError(f"logits processors stage at most {processors.MAX_HIST} history tokens per row: an input of "
+                             f"{n_in} columns on an engine of max_seq_len {S} does not fit")
+        eos = list(eos_ids) if settings["min_length"] or settings["min_new_tokens"] else []
+        self.d_proc.copy_(processors.pack_params(input_len=n_in, eos_ids=eos, **settings))
+        self.d_proc_prompt[:R, :n_in].copy_(prompt_ids.to(torch.int32))
+        self.proc_on = True
+
+    def clear_processors(self):
+        self.proc_on = False
+
+    def process_logits(self, logits, step=False, beam=False):
+        """Apply the set_processors settings in place to rows of fp32 logits: step=False is the first generated token
+        (the prefill logits, nothing generated yet); step=True a decode step, reading the rows' generated ids from
+        token_log (through beam_src for beam rows, which get log-softmax first). A CUDA engine runs the kernel; a CPU
+        engine runs the host statement of the same contract (vitron_b200.processors)."""
+        R = logits.shape[0]
+        state = {}
+        if step:
+            state = dict(token_log=self.token_log[:R], kv_len=self.d_len[:R], prompt_len=self.d_prompt[:R])
+            if beam:
+                state["beam_src"] = self.beam["beam_src"][:R]
+        fn = ops.logits_process if self.device.type == "cuda" else processors.process
+        return fn(logits, self.d_proc, self.d_proc_prompt[:R], logprobs=beam, **state)
+
     def _beam_state(self):
         if self.beam is None:
             R, S, dev = self.max_batch, self.cache.max_seq_len, self.device
@@ -525,20 +573,21 @@ class LlamaEngine:
         if self.beam is None or self.beam_k < 1:
             raise RuntimeError("no beam search is set up on this engine: call start_beam() before beam steps")
 
-    def beam_advance(self, logits, sample=False):
+    def beam_advance(self, logits, sample=False, logprobs=False):
         """The beam step over rows of fp32 logits with the start_beam parameters (sample=True: the beam-sampling step,
-        with the set_sampling parameters too). A CUDA engine runs the kernel; a CPU engine, which runs no kernels of this
-        library, runs the host statement of the same contract (vitron_b200.beam)."""
+        with the set_sampling parameters too; logprobs=True: the rows hold processed log-probabilities). A CUDA engine
+        runs the kernel; a CPU engine, which runs no kernels of this library, runs the host statement of the same
+        contract (vitron_b200.beam)."""
         self._require_beam()
         R = logits.shape[0]
         state = dict({n: t[:R] for n, t in self.beam.items()}, next_src=self.d_src[:R], positions=self.d_pos[:R],
                      kv_len=self.d_len[:R], token_log=self.token_log[:R], prompt_len=self.d_prompt[:R])
         if sample:
             fn = ops.beam_sample_advance if self.device.type == "cuda" else _beam.beam_sample_advance
-            fn(logits, self.beam_k, self.d_beam, self.d_sample, **state)
+            fn(logits, self.beam_k, self.d_beam, self.d_sample, **state, logprobs=logprobs)
         else:
             fn = ops.beam_advance if self.device.type == "cuda" else _beam.beam_advance
-            fn(logits, self.beam_k, self.d_beam, **state)
+            fn(logits, self.beam_k, self.d_beam, **state, logprobs=logprobs)
 
     def start_beam(self, logits, k, max_new_tokens, params, sample=False, searches=1):
         """Beam search over the B prompts of the last prefill: logits [B, V] are its last-token logits, params a
@@ -582,7 +631,10 @@ class LlamaEngine:
         st["beam_score"][:R].copy_(init.reshape(-1))
         for name in ("done", "hyp_count"):
             st[name][:B * searches].zero_()
-        self.beam_advance(logits.float().repeat_interleave(rk, 0).contiguous(), sample=sample)
+        rows = logits.float().repeat_interleave(rk, 0).contiguous()
+        if self.proc_on:     # the first generated token: the processors see the prompt only
+            self.process_logits(rows, beam=True)
+        self.beam_advance(rows, sample=sample, logprobs=self.proc_on)
 
     def start_decode(self, first_tokens, max_new_tokens):
         """first_tokens [B] int64: the token chosen from the prefill logits (already counted as
@@ -603,7 +655,8 @@ class LlamaEngine:
     def decode_steps(self, B, n, use_graph=True, sampled=False):
         """Run n decode steps for slots 0..B-1 (no host sync): greedy, sampled with the set_sampling parameters, or
         (sampled="beam" / "beam_sample") beam-search / beam-sampling steps over the B = searches x num_beams rows of
-        start_beam. The beam modes read their parameters from device buffers: one graph per (rows, mode, k)."""
+        start_beam. The beam modes read their parameters from device buffers: one graph per (rows, mode, k). The logits
+        processors (set_processors) also read theirs from device buffers: one graph more per key with them on."""
         if n <= 0:
             return
         beam_mode = sampled in ("beam", "beam_sample")
@@ -613,7 +666,7 @@ class LlamaEngine:
             for _ in range(n):
                 self._step_kernels(B, sampled)
             return
-        key = (B, sampled, self.beam_k) if beam_mode else (B, bool(sampled))
+        key = (B, sampled, self.beam_k, self.proc_on) if beam_mode else (B, bool(sampled), self.proc_on)
         if key not in self._graphs:
             # warm-up on a side stream (allocator + lazy init), then capture
             s = torch.cuda.Stream(device=self.device)
@@ -632,11 +685,10 @@ class LlamaEngine:
             l0 = ops.launch_count()
             with torch.cuda.graph(g):
                 self._step_kernels(B, sampled)
-            self.launches_per_step = ops.launch_count() - l0
             for t, sv in zip(state, saved):
                 t.copy_(sv)
-            self._graphs[key] = g
-        g = self._graphs[key]
+            self._graphs[key] = (g, ops.launch_count() - l0)
+        g, self.launches_per_step = self._graphs[key]     # graphs with processors launch one kernel more
         for _ in range(n):
             g.replay()
         ops.count_launches(n * self.launches_per_step)

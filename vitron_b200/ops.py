@@ -9,7 +9,7 @@ import struct
 
 import torch
 
-from . import _lib, beam
+from . import _lib, beam, processors
 from .nf4 import NF4Weight
 from ._lib import (ACT_GELU, ACT_NONE, ACT_QUICK_GELU, ACT_RELU, ACT_SILU, GLU_GEGLU, GLU_NONE,
                    GLU_SWIGLU, Epilogue, check)
@@ -647,27 +647,71 @@ def _beam_args(logits, k, params, beam_score, parent, done, beam_src, hyp_score,
 
 
 def beam_advance(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count, hyp_ids,
-                 next_src, positions, kv_len, token_log, prompt_len):
+                 next_src, positions, kv_len, token_log, prompt_len, logprobs=False):
     """One beam-search step for B = rows / k requests (contract in include/vitron_b200.h, statement in
-    vitron_b200.beam): parameters from the device buffer `params` (beam.pack_params), state updated in place."""
+    vitron_b200.beam): parameters from the device buffer `params` (beam.pack_params), state updated in place.
+    logprobs=True: the rows already hold (processed) log-probabilities (logits_process(..., logprobs=True))."""
     args = _beam_args(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
                       hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
-    check(_lib.load().vb200_beam_advance(*args, _stream()), "vb200_beam_advance")
+    name = "vb200_beam_advance_logprobs" if logprobs else "vb200_beam_advance"
+    check(getattr(_lib.load(), name)(*args, _stream()), name)
     _launches[0] += 1
 
 
 def beam_sample_advance(logits, k, params, sample_params, beam_score, parent, done, beam_src, hyp_score, hyp_len,
-                        hyp_seq, hyp_count, hyp_ids, next_src, positions, kv_len, token_log, prompt_len):
+                        hyp_seq, hyp_count, hyp_ids, next_src, positions, kv_len, token_log, prompt_len, logprobs=False):
     """One beam-sampling step (HF 4.31 beam_sample) for B = rows / k searches: beam_advance's arguments plus the device
     buffer `sample_params` (sample_params: temperature, top_k, top_p, seed). Contract in include/vitron_b200.h,
-    statement in vitron_b200.beam.beam_sample_advance."""
+    statement in vitron_b200.beam.beam_sample_advance. logprobs as in beam_advance."""
     _req(sample_params.dtype == torch.uint8 and sample_params.numel() == SAMPLE_PARAMS.size
          and sample_params.is_contiguous() and sample_params.device == logits.device,
          f"sample_params: uint8 [{SAMPLE_PARAMS.size}] sampling buffer on the logits' device")
     args = _beam_args(logits, k, params, beam_score, parent, done, beam_src, hyp_score, hyp_len, hyp_seq, hyp_count,
                       hyp_ids, next_src, positions, kv_len, token_log, prompt_len)
-    check(_lib.load().vb200_beam_sample_advance(*args, sample_params.data_ptr(), _stream()), "vb200_beam_sample_advance")
+    name = "vb200_beam_sample_advance_logprobs" if logprobs else "vb200_beam_sample_advance"
+    check(getattr(_lib.load(), name)(*args, sample_params.data_ptr(), _stream()), name)
     _launches[0] += 1
+
+
+PROC_PARAMS = processors.PARAMS            # vb_proc_params
+proc_params = processors.pack_params       # packed into a CPU uint8 tensor (copy it into the device buffer)
+
+
+def logits_process(logits, params, prompt_ids, token_log=None, kv_len=None, prompt_len=None, beam_src=None,
+                   logprobs=False):
+    """HF 4.31 repetition penalty, no-repeat n-grams, min_length and min_new_tokens, in place on fp32 rows [R, V]
+    (contract in include/vitron_b200.h, statement in vitron_b200.processors): parameters from the device buffer `params`
+    (processors.pack_params), row r's prompt in prompt_ids[r] (int32). Without kv_len / prompt_len no token is generated
+    yet (the prefill logits). beam_src: beam rows read their generated ids through it. logprobs=True writes the rows'
+    log-softmax first (the beam modes)."""
+    lib = _lib.load()
+    _req(logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1, "fp32 logits [R, V]")
+    R, dev = logits.shape[0], logits.device
+    _req(params.dtype == torch.uint8 and params.numel() == processors.PARAMS.size and params.is_contiguous()
+         and params.device == dev, f"params: uint8 [{processors.PARAMS.size}] processor buffer on the logits' device")
+    _req(prompt_ids.dtype == torch.int32 and prompt_ids.dim() == 2 and prompt_ids.stride(1) == 1
+         and prompt_ids.shape[0] >= R and prompt_ids.device == dev,
+         f"prompt_ids: int32 [>= {R}, S] with unit inner stride on the logits' device")
+    _req((kv_len is None) == (prompt_len is None), "kv_len and prompt_len go together")
+    if kv_len is not None:
+        for name, t in (("kv_len", kv_len), ("prompt_len", prompt_len)):
+            _req(t.dtype == torch.int32 and t.dim() == 1 and t.is_contiguous() and t.numel() >= R and t.device == dev,
+                 f"{name}: contiguous int32 [>= {R}] on the logits' device")
+        _req(token_log is not None and token_log.dtype == torch.int64 and token_log.dim() == 2
+             and token_log.stride(1) == 1 and token_log.shape[0] >= R and token_log.device == dev,
+             f"token_log: int64 [>= {R}, S] with unit inner stride on the logits' device")
+    if beam_src is not None:
+        _req(kv_len is not None, "beam_src needs kv_len / prompt_len")
+        _req(beam_src.dtype == torch.int32 and beam_src.dim() == 2 and beam_src.stride(1) == 1
+             and beam_src.shape[0] >= R and beam_src.device == dev,
+             f"beam_src: int32 [>= {R}, S] with unit inner stride on the logits' device")
+    check(lib.vb200_logits_process(logits.data_ptr(), logits.stride(0), R, logits.shape[1], params.data_ptr(),
+                                   prompt_ids.data_ptr(), prompt_ids.stride(0), _ptr(token_log),
+                                   token_log.stride(0) if token_log is not None and kv_len is not None else 0,
+                                   _ptr(beam_src), beam_src.stride(0) if beam_src is not None else 0, _ptr(kv_len),
+                                   _ptr(prompt_len), 1 if logprobs else 0, _stream()), "vb200_logits_process")
+    _launches[0] += 1
+    return logits
 
 
 def patchify(pixels, patch, kpad):

@@ -14,7 +14,7 @@ from types import SimpleNamespace
 
 import torch
 
-from . import beam, ops
+from . import beam, ops, processors
 from .module_face import ModuleFace
 from .adapters import RegionExtractor, VisionProjector
 from .llama import LlamaConfig, LlamaEngine
@@ -493,7 +493,8 @@ class VitronLlamaForCausalLM(ModuleFace):
     def generate(self, input_ids=None, images=None, regions=None, do_sample=False, temperature=1.0, top_p=None,
                  top_k=None, max_new_tokens=32, use_cache=True, stopping_criteria=None, attention_mask=None,
                  eos_token_id=None, pad_token_id=None, inputs=None, sync_every=16, num_beams=1, length_penalty=1.0,
-                 early_stopping=False, num_return_sequences=1, **kwargs):
+                 early_stopping=False, num_return_sequences=1, repetition_penalty=1.0, no_repeat_ngram_size=0,
+                 min_length=0, min_new_tokens=0, **kwargs):
         """Greedy (or sampled) decoding with the reference call signature
         (inference_image.py:53-61, app.py:562-571). Returns input_ids followed by the generated ids,
         like HF `generate` for decoder-only models.
@@ -516,7 +517,15 @@ class VitronLlamaForCausalLM(ModuleFace):
         num_return_sequences = r runs r independent searches per request and returns each one's best hypothesis:
         [B * r, input_len + gen_len], request-major; B * r * num_beams rows must fit the engine's max_batch. The seed is
         drawn from torch's default CPU generator as in sampling; prefill, page sharing, sync_every and
-        stopping_criteria behave as in beam search."""
+        stopping_criteria behave as in beam search.
+
+        repetition_penalty, no_repeat_ngram_size, min_length and min_new_tokens are HF 4.31's logits processors, stated
+        in vitron_b200.processors and enabled by 4.31's rules (repetition_penalty != 1.0, no_repeat_ngram_size > 0, and
+        with an EOS id, min_length > 0 / min_new_tokens > 0; min_length counts input_ids.shape[1] + generated tokens).
+        They see input_ids as 4.31 does (image and region sentinels one position each, left padding included) followed by
+        the generated ids, and apply in every mode, first token included: to the logits before the arg-max or the
+        sampler's warpers, and in the beam modes to the log-probabilities before the beam scores are added. They run on
+        the device inside the graphed decode step. Sentinel ids are never penalised or banned (4.31 fails on them)."""
         if input_ids is None:
             input_ids = inputs
         eos = self.config.eos_token_id if eos_token_id is None else eos_token_id
@@ -535,6 +544,9 @@ class VitronLlamaForCausalLM(ModuleFace):
         if beam_sample and B * num_return_sequences * num_beams > self.engine.max_batch:
             raise ValueError(f"batch {B} x num_return_sequences {num_return_sequences} x num_beams {num_beams} = "
                              f"{B * num_return_sequences * num_beams} rows > engine max_batch {self.engine.max_batch}")
+        eos_list = sorted(eos_set) if not isinstance(eos, (list, tuple)) else [int(e) for e in eos]
+        proc_settings, proc_on = processors.check_settings(repetition_penalty, no_repeat_ngram_size, min_length,
+                                                           min_new_tokens, eos_list)
         self._kv_segments = None          # the prefill and decode below overwrite the cache: every handle becomes stale
         if images is not None:
             _, _, am, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(
@@ -545,14 +557,20 @@ class VitronLlamaForCausalLM(ModuleFace):
             am = attention_mask
         embeds, lens, _ = self._right_pad(embeds, am)
         eng = self.engine
+        if proc_on:    # every engine row gets its request's raw input_ids row (a beam row its search's request)
+            rows = num_beams * (num_return_sequences if beam_sample else 1) if num_beams > 1 else 1
+            eng.set_processors(input_ids.detach().cpu().repeat_interleave(rows, 0), eos_ids=eos_list, **proc_settings)
+        else:
+            eng.clear_processors()
         logits = eng.prefill(embeds, lens)
         if do_sample:
             seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64)) & (2 ** 64 - 1)
             eng.set_sampling(temperature, top_k, top_p, seed)
         if beam_search or beam_sample:
-            eos_list = sorted(eos_set) if not isinstance(eos, (list, tuple)) else [int(e) for e in eos]
             return self._beam_search(input_ids, logits, num_beams, num_return_sequences, length_penalty, early_stopping,
                                      eos_list, pad, max_new_tokens, stopping_criteria, sync_every, sample=beam_sample)
+        if proc_on:
+            eng.process_logits(logits)                                # generated token 0: nothing generated yet
         if do_sample:
             first = eng.sample_advance(logits)                        # generated token 0: Philox step 0
         else:
