@@ -1,5 +1,7 @@
 """Kernel-level numerics: every C-ABI entry point against a plain torch fp32 reference of the same
-op on the same seeded inputs (these are floating-point kernels: tolerance stated per test)."""
+op on the same seeded inputs (these are floating-point kernels: tolerance stated per test). The tolerances here are
+fixed and several times the bf16 rounding of the output; the GEMM above 64 rows, the convolution and GroupNorm are pinned
+against float64 with derived bounds, on every planner branch, in tests/test_gemm_conv_groupnorm_gpu.py."""
 import math
 
 import pytest

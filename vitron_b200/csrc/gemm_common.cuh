@@ -129,7 +129,7 @@ __device__ __forceinline__ void reduce_item(const float* __restrict__ ws, int sp
       if (oc + j < n_out_total) dst[j] = v[j];
   } else {
     bf16* dst = reinterpret_cast<bf16*>(out) + row * ldo + oc;
-    if (oc + 8 <= n_out_total && (ldo & 7) == 0) {
+    if (oc + 8 <= n_out_total && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {   // out may be a view at any column
       *reinterpret_cast<uint4*>(dst) = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]),
                                                   pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
     } else {

@@ -318,19 +318,38 @@ static int launch_rownorm(const void* x, long long ldx, const void* w, const voi
 //   kernels, 3.5 ms of a 25 ms UNet forward; a coalesced stats / apply pair with a last-CTA finaliser measured 15.7 +
 //   16.6 us per GroupNorm — both launches are latency chains (launch, L2 round trips, atomics, fence) longer than
 //   the data movement, so the fix is one launch and one read, not faster loops.
-__device__ __forceinline__ void gn_accumulate(const uint4 u, float (&s)[8], float (&q)[8]) {
-  float2 f;
-  f = unpack_bf16(u.x); s[0] += f.x; q[0] += f.x * f.x; s[1] += f.y; q[1] += f.y * f.y;
-  f = unpack_bf16(u.y); s[2] += f.x; q[2] += f.x * f.x; s[3] += f.y; q[3] += f.y * f.y;
-  f = unpack_bf16(u.z); s[4] += f.x; q[4] += f.x * f.x; s[5] += f.y; q[5] += f.y * f.y;
-  f = unpack_bf16(u.w); s[6] += f.x; q[6] += f.x * f.x; s[7] += f.y; q[7] += f.y * f.y;
+// Two sets of sums per channel: of x and x^2 (s, q), and of d = x - K and d^2 (ds, dq) around a pivot K per (sample,
+// group), the group's first channel in the sample's first row. var = E[x^2] - mean^2 cancels in fp32 when the group mean
+// is large next to its spread (at |mean| / std = 256, rstd came out 2e-2 off); var = E[d^2] - E[d]^2 does not. The
+// statistics take the plain sums when |mean| <= 2 std and the pivot sums otherwise (gn_stats).
+__device__ __forceinline__ void gn_accumulate(const uint4 u, const float (&k)[8], float (&s)[8], float (&q)[8],
+                                              float (&ds)[8], float (&dq)[8]) {
+  const uint32_t uu[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = unpack_bf16(uu[j]);
+    s[2 * j] += f.x; q[2 * j] += f.x * f.x; s[2 * j + 1] += f.y; q[2 * j + 1] += f.y * f.y;
+    const float d0 = f.x - k[2 * j], d1 = f.y - k[2 * j + 1];
+    ds[2 * j] += d0; dq[2 * j] += d0 * d0; ds[2 * j + 1] += d1; dq[2 * j + 1] += d1 * d1;
+  }
+}
+
+// (mean, rstd) of a group from its plain sums (sum, sq) and its pivot sums (dsum, dsq) around k over cnt elements
+__device__ __forceinline__ float2 gn_stats(float sum, float sq, float dsum, float dsq, float k, float cnt, float eps) {
+  const float mean = sum / cnt;
+  const float dm = dsum / cnt;
+  const float dvar = fmaxf(dsq / cnt - dm * dm, 0.f);
+  // (__fmul_rn: the test must not change how the plain formula below is contracted)
+  if (__fmul_rn(mean, mean) > 4.f * dvar) return make_float2(k + dm, rsqrtf(dvar + eps));
+  const float rstd = rsqrtf(fmaxf(sq / cnt - mean * mean, 0.f) + eps);
+  return make_float2(mean, rstd);
 }
 
 // The CTAs of a sample publish their group partial sums in slots of their own (no atomics) and every CTA adds the slots
 // of its sample in one fixed order, so the statistics — and everything downstream of them — are bit-identical from run
 // to run.
 struct GnWs {
-  float* sums;      // [n * ctas per sample][groups][2]: one slot per CTA, overwritten by every launch
+  float* sums;      // [n * ctas per sample][groups][4]: one slot per CTA, overwritten by every launch
   int* arrived;     // [n]  CTAs of the sample that published their sums
   int* readers;     // [n]  CTAs of the sample that consumed the sums (the last one resets both counters)
 };
@@ -379,7 +398,8 @@ __global__ void __launch_bounds__(512)
 gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ b, bf16* __restrict__ out,
                   GnWs ws, int spatial, int c, int groups, int rows_per_cta, int rpp, float eps) {
   extern __shared__ __align__(128) uint8_t gsm[];
-  __shared__ float gsum[1024];                                                        // [groups][2] when the sample is one CTA
+  __shared__ float gsum[1024];                                                        // [groups][2]: sums, then (mean, rstd)
+  __shared__ float gpiv[512];                                                         // [groups] pivots
   __shared__ __align__(8) uint64_t slab_bar;
   float* part = reinterpret_cast<float*>(gsm);                                        // [rpp][c][2], later aff[2][c]
   uint4* slab = reinterpret_cast<uint4*>(gsm + static_cast<size_t>(rpp) * c * 2 * sizeof(float));  // [rows][c/8]
@@ -398,22 +418,29 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
   }
   __syncthreads();
   pdl_wait();  // nothing of the predecessor's output has been touched above
-  float s[8], q[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
-  if (CACHED) {
+  if (CACHED && threadIdx.x == 0) {
     // the CTA's slab is ONE contiguous range of global memory: the TMA unit copies it into shared memory in 32 KB
     // pieces (all in flight at once: the register-load loop this replaces kept ~30 KB per SM in flight and was latency
     // bound), every thread then accumulates its fixed 8-channel column out of shared memory
-    if (threadIdx.x == 0) {
-      const uint32_t total = static_cast<uint32_t>(rows) * c * 2;
-      mbar_arrive_expect_tx(&slab_bar, total);
-      const uint8_t* src = reinterpret_cast<const uint8_t*>(x + (static_cast<size_t>(n) * spatial + r0) * c);
-      for (uint32_t o = 0; o < total; o += 32768) bulk_copy_g2s(reinterpret_cast<uint8_t*>(slab) + o, src + o, min(32768u, total - o), &slab_bar);
-    }
+    const uint32_t total = static_cast<uint32_t>(rows) * c * 2;
+    mbar_arrive_expect_tx(&slab_bar, total);
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(x + (static_cast<size_t>(n) * spatial + r0) * c);
+    for (uint32_t o = 0; o < total; o += 32768) bulk_copy_g2s(reinterpret_cast<uint8_t*>(slab) + o, src + o, min(32768u, total - o), &slab_bar);
+  }
+  const int cpg = c / groups;
+  const bf16* xn = x + static_cast<size_t>(n) * spatial * c;   // row 0 of the sample: the group pivots
+  float s[8], q[8], ds[8], dq[8], kp[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    s[j] = q[j] = ds[j] = dq[j] = 0.f;
+    kp[j] = active ? __bfloat162float(xn[(my_vec * 8 + j) / cpg * cpg]) : 0.f;
+  }
+  // the statistics need the pivots again; read them now, before any CTA of the sample can overwrite row 0 (in place)
+  for (int g = threadIdx.x; g < groups; g += blockDim.x) gpiv[g] = __bfloat162float(xn[g * cpg]);
+  if (CACHED) {
     mbar_wait(&slab_bar, 0);
     if (active)
-      for (int r = my_row; r < rows; r += rpp) gn_accumulate(slab[r * vec_per_row + my_vec], s, q);
+      for (int r = my_row; r < rows; r += rpp) gn_accumulate(slab[r * vec_per_row + my_vec], kp, s, q, ds, dq);
   } else if (active) {
     int r = my_row;
     for (; r + 7 * rpp < rows; r += 8 * rpp) {  // eight independent 16-byte loads in flight
@@ -421,42 +448,52 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
 #pragma unroll
       for (int k = 0; k < 8; ++k) u[k] = __ldg(reinterpret_cast<const uint4*>(xb + static_cast<size_t>(r + k * rpp) * c));
 #pragma unroll
-      for (int k = 0; k < 8; ++k) gn_accumulate(u[k], s, q);
+      for (int k = 0; k < 8; ++k) gn_accumulate(u[k], kp, s, q, ds, dq);
     }
-    for (; r < rows; r += rpp) gn_accumulate(__ldg(reinterpret_cast<const uint4*>(xb + static_cast<size_t>(r) * c)), s, q);
+    for (; r < rows; r += rpp) gn_accumulate(__ldg(reinterpret_cast<const uint4*>(xb + static_cast<size_t>(r) * c)), kp, s, q, ds, dq);
   }
-  if (active) {
-    float* mine = part + (static_cast<size_t>(my_row) * c + my_vec * 8) * 2;
-#pragma unroll
-    for (int j = 0; j < 8; j += 2)
-      *reinterpret_cast<float4*>(mine + j * 2) = make_float4(s[j], q[j], s[j + 1], q[j + 1]);
-  }
-  __syncthreads();
-  const int cpg = c / groups;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;  // blockDim is a multiple of 32
   const int ctas = gridDim.x;
-  const float* gs = ws.sums + static_cast<size_t>(n) * ctas * groups * 2;           // the slots of this sample
-  float* gs_mine = ws.sums + (static_cast<size_t>(n) * ctas + blockIdx.x) * groups * 2;  // this CTA's slot
-  for (int g = warp; g < groups; g += nwarps) {
-    float as = 0.f, aq = 0.f;
-    const int items = rpp * cpg;
-    for (int e = lane; e < items; e += 32) {
-      const int rr = e / cpg, ch = g * cpg + (e - rr * cpg);
-      const float2 v = *reinterpret_cast<const float2*>(part + (static_cast<size_t>(rr) * c + ch) * 2);
-      as += v.x;
-      aq += v.y;
+  const float cnt = static_cast<float>(cpg) * static_cast<float>(spatial);
+  const float* gs = ws.sums + static_cast<size_t>(n) * ctas * groups * 4;           // the slots of this sample
+  float* gs_mine = ws.sums + (static_cast<size_t>(n) * ctas + blockIdx.x) * groups * 4;  // this CTA's slot [groups][4]
+  // the CTA's group sums, plain (pass 0) then pivot (pass 1), through the same [rpp][c][2] staging area; a group's sums are
+  // reduced by the same warp in both passes, so with one CTA per sample its lane 0 holds all four and stores (mean, rstd)
+  for (int pass = 0; pass < 2; ++pass) {
+    if (active) {
+      float* mine = part + (static_cast<size_t>(my_row) * c + my_vec * 8) * 2;
+#pragma unroll
+      for (int j = 0; j < 8; j += 2)
+        *reinterpret_cast<float4*>(mine + j * 2) = pass == 0 ? make_float4(s[j], q[j], s[j + 1], q[j + 1])
+                                                             : make_float4(ds[j], dq[j], ds[j + 1], dq[j + 1]);
     }
-    as = warp_sum(as);
-    aq = warp_sum(aq);
-    if (lane == 0) {
-      if (ctas > 1) {
-        gs_mine[g * 2] = as;
-        gs_mine[g * 2 + 1] = aq;
-      } else {  // the whole sample is this CTA: no global round trip
-        gsum[g * 2] = as;
-        gsum[g * 2 + 1] = aq;
+    __syncthreads();
+    for (int g = warp; g < groups; g += nwarps) {
+      float as = 0.f, aq = 0.f;
+      const int items = rpp * cpg;
+      for (int e = lane; e < items; e += 32) {
+        const int rr = e / cpg, ch = g * cpg + (e - rr * cpg);
+        const float2 v = *reinterpret_cast<const float2*>(part + (static_cast<size_t>(rr) * c + ch) * 2);
+        as += v.x;
+        aq += v.y;
+      }
+      as = warp_sum(as);
+      aq = warp_sum(aq);
+      if (lane == 0) {
+        if (ctas > 1) {
+          gs_mine[g * 4 + 2 * pass] = as;
+          gs_mine[g * 4 + 2 * pass + 1] = aq;
+        } else if (pass == 0) {  // the whole sample is this CTA: no global round trip
+          gsum[g * 2] = as;
+          gsum[g * 2 + 1] = aq;
+        } else {
+          const float2 st = gn_stats(gsum[g * 2], gsum[g * 2 + 1], as, aq, gpiv[g], cnt, eps);
+          gsum[g * 2] = st.x;
+          gsum[g * 2 + 1] = st.y;
+        }
       }
     }
+    __syncthreads();   // pass 1 overwrites the staging area
   }
   // ---- the CTAs of this sample meet: publish, then wait until all have published
   if (ctas > 1) {
@@ -468,25 +505,30 @@ gn_onepass_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const 
     }
   }
   __syncthreads();
-  // ---- group sums of the sample = sum of its CTAs' slots -> gsum, in a fixed order (lane l adds slots l, l + 32, ...,
-  // then a fixed shuffle tree); then the per-channel affine into smem (`part` is free: every warp passed the barrier
-  // above after its reads)
+  // ---- group sums of the sample = sum of its CTAs' slots, in a fixed order (lane l adds slots l, l + 32, ..., then a
+  // fixed shuffle tree) -> (mean, rstd) in gsum; then the per-channel affine into smem (`part` is free: every warp passed
+  // the barrier above after its reads)
   if (ctas > 1) {
-    for (int i = warp; i < groups * 2; i += nwarps) {
-      float a = 0.f;
-      for (int k = lane; k < ctas; k += 32) a += __ldcg(gs + static_cast<size_t>(k) * groups * 2 + i);
-      a = warp_sum(a);
-      if (lane == 0) gsum[i] = a;
+    for (int g = warp; g < groups; g += nwarps) {
+      float a[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int k = lane; k < ctas; k += 32) {
+        const float4 v = __ldcg(reinterpret_cast<const float4*>(gs + (static_cast<size_t>(k) * groups + g) * 4));
+        a[0] += v.x; a[1] += v.y; a[2] += v.z; a[3] += v.w;
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = warp_sum(a[i]);
+      if (lane == 0) {
+        const float2 st = gn_stats(a[0], a[1], a[2], a[3], gpiv[g], cnt, eps);
+        gsum[g * 2] = st.x;
+        gsum[g * 2 + 1] = st.y;
+      }
     }
     __syncthreads();
   }
-  const float cnt = static_cast<float>(cpg) * static_cast<float>(spatial);
   float* aff = part;  // [2][c]
   for (int ch = threadIdx.x; ch < c; ch += blockDim.x) {
     const int g = ch / cpg;
-    const float sum = gsum[g * 2], sq = gsum[g * 2 + 1];
-    const float mean = sum / cnt;
-    const float rstd = rsqrtf(fmaxf(sq / cnt - mean * mean, 0.f) + eps);
+    const float mean = gsum[g * 2], rstd = gsum[g * 2 + 1];
     const float sc = rstd * __bfloat162float(w[ch]);
     aff[ch] = sc;
     aff[c + ch] = __bfloat162float(b[ch]) - mean * sc;
@@ -557,7 +599,7 @@ extern "C" int vb200_layernorm(const void* x, int64_t ldx, const void* weight, c
   return launch_rownorm<true>(x, ldx, weight, bias, out, ldo, rows, d, eps, stream);
 }
 
-constexpr int GN_DYN_SMEM_MAX = 220 * 1024;  // dynamic smem budget of gn_onepass_kernel (+ 5 KB static <= 227 KB)
+constexpr int GN_DYN_SMEM_MAX = 220 * 1024;  // dynamic smem budget of gn_onepass_kernel (+ 6 KB static <= 227 KB)
 
 static size_t gn_align16(size_t v) { return (v + 15) & ~static_cast<size_t>(15); }
 
@@ -572,7 +614,7 @@ extern "C" size_t vb200_groupnorm_workspace_size(int64_t n, int64_t groups, int6
   (void)c;
   if (n > GN_MAX_N) n = GN_MAX_N;
   const int64_t ctas = n > vb_num_sms() ? n : vb_num_sms();
-  return GN_COUNTER_BYTES + gn_align16(static_cast<size_t>(ctas) * groups * 2 * sizeof(float));
+  return GN_COUNTER_BYTES + gn_align16(static_cast<size_t>(ctas) * groups * 4 * sizeof(float));
 }
 
 template <int ACT, bool CACHED>
@@ -583,7 +625,7 @@ static int gn_launch(const bf16* x, const bf16* w, const bf16* b, bf16* out, GnW
   if (!attr_set) {
     // opt in once per instantiation, whatever the first launch needs: the default limit of 48 KB counts the kernel's 4 KB of
     // STATIC shared memory too (a first launch with exactly 48 KB of dynamic smem failed with "invalid argument").
-    // 227 KB per CTA minus the static part (gsum + flags: 5 KB)
+    // 227 KB per CTA minus the static part (gsum + pivots + barrier: 6 KB)
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GN_DYN_SMEM_MAX);
     if (e != cudaSuccess) { vb_set_last_error(e); return VB_ERR_CUDA; }
     attr_set = true;
