@@ -140,7 +140,9 @@ int vb200_conv_nhwc_direct(const void* X, const void* Wt, const void* bias, void
 
 /* ---- normalisation (norm.cu) ----------------------------------------------------------------
  * rmsnorm: HF LlamaRMSNorm (fp32 statistics). layernorm: nn.LayerNorm. groupnorm: nn.GroupNorm
- * over NHWC [n, spatial, c] (+ optional SiLU / ReLU), i2vgen util.py:640-655,1358-1375. */
+ * over NHWC [n, spatial, c] (+ optional SiLU / ReLU), i2vgen util.py:640-655,1358-1375.
+ * rmsnorm / layernorm: d, ldx and ldo multiples of 8 and x, weight, bias and out 16-byte aligned (VB_ERR_ARG otherwise),
+ * d <= 16384 (VB_ERR_UNSUPPORTED above). row_rstd: the same for d, ldx and x. */
 int vb200_rmsnorm(const void* x, int64_t ldx, const void* weight, void* out, int64_t ldo,
                   int64_t rows, int64_t d, float eps, cudaStream_t stream);
 /* out[row] = rsqrt(mean(x_row^2) + eps), fp32: the rowscale of the RMSNorm-folded GEMMs (prefill) */
@@ -412,14 +414,14 @@ int vb200_patchify(const void* pixels, int in_is_fp32, void* out, int64_t nb, in
 int vb200_vit_embed_ln(const void* patch_out, const void* cls, const void* pos, const void* ln_w,
                        const void* ln_b, void* out, int64_t nb, int64_t npatch, int64_t d,
                        float eps, cudaStream_t stream);
-/* nearest x2 upsample NHWC (util.py:579-607) */
+/* nearest x2 upsample NHWC (util.py:579-607); x and out 16-byte aligned */
 int vb200_upsample2x_nhwc(const void* x, void* out, int64_t nb, int64_t h, int64_t w, int64_t c,
                           cudaStream_t stream);
-/* out = a + b (bf16, n elements), with optional broadcast period for b */
+/* out = a + b (bf16, n elements), with optional broadcast period for b; a, b and out 16-byte aligned */
 int vb200_add_bf16(const void* a, const void* b, void* out, int64_t n, int64_t b_period,
                    cudaStream_t stream);
 /* out[row] = x[row] + table[(row / group_rows) % period] — LanguageBind temporal_embedding add on
- * '(b t) n d' rows (modeling_video.py:110-113) */
+ * '(b t) n d' rows (modeling_video.py:110-113); x, table and out contiguous and 16-byte aligned */
 int vb200_add_rowgroup(const void* x, const void* table, void* out, int64_t rows, int64_t d,
                        int64_t group_rows, int64_t period, cudaStream_t stream);
 /* classifier-free guidance combine u + s (y - u) in fp32 (diffusion_ddim.py:156-158) */
@@ -434,7 +436,8 @@ int vb200_region_mask_pool(const void* feats, const float* boxes, void* out, int
  * cleared (seem.py:569-574, attention_data_struct.py:187). */
 int vb200_seem_attn_mask(const float* mask_logits, uint8_t* out_mask, int64_t Q, int64_t H,
                          int64_t W, int64_t h2, int64_t w2, cudaStream_t stream);
-/* F.interpolate(mode="bilinear", align_corners=False) of NHWC bf16 images [nb, H, W, C] -> [nb, h2, w2, C] (C % 8 == 0).
+/* F.interpolate(mode="bilinear", align_corners=False) of NHWC bf16 images [nb, H, W, C] -> [nb, h2, w2, C] (C % 8 == 0,
+ * x and out 16-byte aligned).
  * SEEM inference path without aux outputs: mask_features resized once per feature level so that the attention-mask logits
  * of seem.py:569-574 (bilinear of einsum('bqc,bchw->bqhw')) become one small GEMM per layer (bilinear is linear). */
 int vb200_resize_bilinear_nhwc(const void* x, void* out, int64_t nb, int64_t H, int64_t W, int64_t C,
@@ -442,7 +445,8 @@ int vb200_resize_bilinear_nhwc(const void* x, void* out, int64_t nb, int64_t H, 
 
 /* out = softmax over the last dim of fp32 x [rows, n] (row stride ldx) -> bf16 [rows, n] (row stride ldo): the
  * single-head c-channel attention of the first-stage VAE's AttnBlock (i2vgen-xl tools/modules/autoencoder.py:418-442),
- * whose QK^T and PV are vb200_gemm_bf16 calls. */
+ * whose QK^T and PV are vb200_gemm_bf16 calls. -inf entries get probability 0, like torch.softmax; a row with at least
+ * one finite entry (and no +inf or NaN) sums to 1, a row of only -inf comes out NaN, as in torch. */
 int vb200_softmax_rows(const float* x, int64_t ldx, void* out, int64_t ldo, int64_t rows, int64_t n,
                        cudaStream_t stream);
 

@@ -522,6 +522,52 @@ def test_argument_validation_of_the_widened_entry_points(lib):
     assert lib.vb200_layernorm_add(p, 64, p, None, None, 0, p, 64, 4, 4096, 1e-5, None) == ERR_ARG  # d > 2048
     assert lib.vb200_im2col_nchw(p, 1, p, 1, 3, 32, 32, 7, 4, 2, 8, 8, 100, None) == ERR_ARG        # kpad < c*k*k / not % 8
     assert lib.vb200_softmax_rows(None, 8, p, 8, 1, 8, None) == ERR_ARG
+    # 16-byte vector loads and stores: a pointer 2 bytes off (e.g. the row view x[:, 1:]) is refused, whichever it is
+    q = p + 2
+    for args in ((q, p, p, p), (p, q, p, p), (p, p, q, p), (p, p, p, q)):
+        x, w, b, o = args
+        assert lib.vb200_layernorm(x, 64, w, b, o, 64, 4, 64, 1e-5, None) == ERR_ARG, args
+        if b == p:
+            assert lib.vb200_rmsnorm(x, 64, w, o, 64, 4, 64, 1e-5, None) == ERR_ARG, args
+    assert lib.vb200_layernorm(p, 64, p, None, q, 64, 4, 64, 1e-5, None) == ERR_ARG
+    assert lib.vb200_row_rstd(q, 64, p, 4, 64, 1e-5, None) == ERR_ARG
+    for x, o in ((q, p), (p, q)):
+        assert lib.vb200_upsample2x_nhwc(x, o, 1, 4, 4, 64, None) == ERR_ARG
+        assert lib.vb200_resize_bilinear_nhwc(x, o, 1, 4, 4, 64, 8, 8, None) == ERR_ARG
+    for a, b, o in ((q, p, p), (p, q, p), (p, p, q)):
+        assert lib.vb200_add_bf16(a, b, o, 64, 0, None) == ERR_ARG
+        assert lib.vb200_add_rowgroup(a, b, o, 4, 64, 2, 2, None) == ERR_ARG
     m3 = (C.c_float * 3)(0.5, 0.5, 0.5)
     assert lib.vb200_preprocess_frames(p, p, 1, 32, 32, 224, 224, 10, 0, 224, 224, 1, 1, m3, m3, 1, 0, 0, None) == ERR_ARG  # crop outside
     assert lib.vb200_preprocess_frames(p, p, 1, 32, 32, 224, 224, 0, 0, 224, 224, 1, 1, m3, m3, 5, 0, 0, None) == ERR_ARG   # unknown mode
+
+
+def test_outputs_that_are_not_row_views_are_refused(lib):
+    """An out= (or in-place) tensor whose rows do not share one stride cannot be handed to a kernel as [rows, d]: a
+    reshape would copy it, the kernel would write the copy and the caller's tensor would never change. The ops raise
+    ValueError before any library call (CPU tensors: nothing here reaches a device)."""
+    import torch
+    from vitron_b200 import ops
+    BF = torch.bfloat16
+    x = torch.zeros((2, 5, 64), dtype=BF)
+    w, b = torch.ones((64,), dtype=BF), torch.zeros((64,), dtype=BF)
+    buf = torch.zeros((2, 8, 64), dtype=BF)
+    bad = buf[:, :5]                                      # [B, S, d] slice of a longer sequence buffer
+    with pytest.raises(ValueError):
+        ops.rmsnorm(x, w, 1e-6, out=bad)
+    with pytest.raises(ValueError):
+        ops.layernorm(x, w, b, 1e-5, out=bad)
+    with pytest.raises(ValueError):
+        ops.layernorm_add(x, w, b, None, 1e-5, out=bad)
+    with pytest.raises(ValueError):
+        ops.gemm(x, torch.zeros((64, 64), dtype=BF), out=bad)
+    with pytest.raises(ValueError):
+        ops.rope_kv_append(bad, torch.zeros((10,), dtype=torch.int32), 1, 64, 1e4)
+    with pytest.raises(ValueError):
+        ops.add_rowgroup(x.reshape(10, 64), torch.zeros((2, 64), dtype=BF), 5, 2, out=bad.reshape(2, 5, 64)[0])
+    with pytest.raises(ValueError):
+        ops.add_rowgroup(x.reshape(10, 64), torch.zeros((2, 64), dtype=BF), 5, 2, out=torch.zeros((10, 64)))
+    # a 3-D view whose rows do share one stride is fine: the reshape check is on views, not on dimensions
+    assert ops._out_rows2d(buf[:1, :5])[1] == 64 and ops._out_rows2d(buf[:, :5][:, :, :32].contiguous())[1] == 32
+    with pytest.raises(ValueError):
+        ops._out_rows2d(buf[:, :5, :32])

@@ -1,7 +1,9 @@
 """Kernel-level numerics: every C-ABI entry point against a plain torch fp32 reference of the same
 op on the same seeded inputs (these are floating-point kernels: tolerance stated per test). The tolerances here are
 fixed and several times the bf16 rounding of the output; the GEMM above 64 rows, the convolution and GroupNorm are pinned
-against float64 with derived bounds, on every planner branch, in tests/test_gemm_conv_groupnorm_gpu.py."""
+against float64 with derived bounds, on every planner branch, in tests/test_gemm_conv_groupnorm_gpu.py, and the row norms,
+row_rstd, layernorm_add, vit_embed_ln, the row softmax and the FocalNet / ViT glue (dwconv, colmean, focal_modulate,
+mul_rows, add, add_rowgroup, upsample2x) in tests/test_norms_softmax_focal_gpu.py."""
 import math
 
 import pytest

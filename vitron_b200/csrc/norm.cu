@@ -277,11 +277,14 @@ rownorm_warp4_kernel(const bf16* __restrict__ x, long long ldx, const bf16* __re
   }
 }
 
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 template <bool LAYER>
 static int launch_rownorm(const void* x, long long ldx, const void* w, const void* b, void* out,
                           long long ldo, long long rows, long long d, float eps, cudaStream_t st) {
   if (rows <= 0) return VB_OK;
   if (d % 8 != 0 || ldx % 8 != 0 || ldo % 8 != 0) return VB_ERR_ARG;
+  if (!aligned16(x) || !aligned16(w) || !aligned16(b) || !aligned16(out)) return VB_ERR_ARG;
   const bf16* xp = reinterpret_cast<const bf16*>(x);
   const bf16* wp = reinterpret_cast<const bf16*>(w);
   const bf16* bp = reinterpret_cast<const bf16*>(b);
@@ -584,7 +587,7 @@ extern "C" int vb200_rmsnorm(const void* x, int64_t ldx, const void* weight, voi
 
 extern "C" int vb200_row_rstd(const void* x, int64_t ldx, float* out, int64_t rows, int64_t d, float eps,
                               cudaStream_t stream) {
-  VB_CHECK_ARG(x && out && rows >= 0 && d > 0 && d % 8 == 0 && ldx % 8 == 0);
+  VB_CHECK_ARG(x && out && rows >= 0 && d > 0 && d % 8 == 0 && ldx % 8 == 0 && aligned16(x));
   if (rows == 0) return VB_OK;
   row_rstd_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, stream>>>(reinterpret_cast<const bf16*>(x), ldx, out,
                                                                              rows, static_cast<int>(d), eps);

@@ -268,6 +268,8 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   float m = -INFINITY, s = 0.f;
   for (int i = threadIdx.x; i < n; i += 256) {
     const float v = xr[i];
+    // a -inf adds nothing to the sum; taken into the online update while m is still -inf, it would make m - mn NaN
+    if (v == -INFINITY) continue;
     const float mn = fmaxf(m, v);
     s = s * __expf(m - mn) + __expf(v - mn);
     m = mn;
@@ -295,6 +297,8 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
 }  // namespace vb
 
 using namespace vb;
+
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 extern "C" int vb200_softmax_rows(const float* x, int64_t ldx, void* out, int64_t ldo, int64_t rows, int64_t n,
                                   cudaStream_t stream) {
@@ -334,7 +338,7 @@ extern "C" int vb200_vit_embed_ln(const void* patch_out, const void* cls, const 
 
 extern "C" int vb200_upsample2x_nhwc(const void* x, void* out, int64_t nb, int64_t h, int64_t w, int64_t c,
                                      cudaStream_t stream) {
-  VB_CHECK_ARG(x && out && nb > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0);
+  VB_CHECK_ARG(x && out && nb > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0 && aligned16(x) && aligned16(out));
   const long long total = nb * 2 * h * 2 * w * (c / 8);
   upsample2x_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), (int)h, (int)w, (int)(c / 8), total);
@@ -345,6 +349,7 @@ extern "C" int vb200_upsample2x_nhwc(const void* x, void* out, int64_t nb, int64
 extern "C" int vb200_add_bf16(const void* a, const void* b, void* out, int64_t n, int64_t b_period,
                               cudaStream_t stream) {
   VB_CHECK_ARG(a && b && out && n >= 0 && n % 8 == 0 && b_period % 8 == 0);
+  VB_CHECK_ARG(aligned16(a) && aligned16(b) && aligned16(out));
   if (n == 0) return VB_OK;
   add_kernel<<<static_cast<unsigned>((n / 8 + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const uint4*>(a), reinterpret_cast<const uint4*>(b), reinterpret_cast<uint4*>(out), n / 8,
@@ -356,6 +361,7 @@ extern "C" int vb200_add_bf16(const void* a, const void* b, void* out, int64_t n
 extern "C" int vb200_add_rowgroup(const void* x, const void* table, void* out, int64_t rows, int64_t d,
                                   int64_t group_rows, int64_t period, cudaStream_t stream) {
   VB_CHECK_ARG(x && table && out && rows >= 0 && d > 0 && d % 8 == 0 && group_rows > 0 && period > 0);
+  VB_CHECK_ARG(aligned16(x) && aligned16(table) && aligned16(out));
   if (rows == 0) return VB_OK;
   const long long nvec = rows * (d / 8);
   add_rowgroup_kernel<<<static_cast<unsigned>((nvec + 255) / 256), 256, 0, stream>>>(
@@ -397,6 +403,7 @@ extern "C" int vb200_seem_attn_mask(const float* mask_logits, uint8_t* out_mask,
 extern "C" int vb200_resize_bilinear_nhwc(const void* x, void* out, int64_t nb, int64_t H, int64_t W, int64_t C, int64_t h2,
                                           int64_t w2, cudaStream_t stream) {
   VB_CHECK_ARG(x && out && nb > 0 && H > 0 && W > 0 && C > 0 && (C % 8) == 0 && h2 > 0 && w2 > 0);
+  VB_CHECK_ARG(aligned16(x) && aligned16(out));
   const long long total = nb * h2 * w2 * (C / 8);
   resize_bilinear_nhwc_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(out), (int)nb, (int)H, (int)W, (int)C, (int)h2, (int)w2);

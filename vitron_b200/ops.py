@@ -119,11 +119,25 @@ def _req(cond, msg):
 
 
 def _rows2d(x):
-    """View x as [rows, d] with unit inner stride; returns (tensor2d, ld)."""
+    """An input x as [rows, d] with unit inner stride; returns (tensor2d, ld). x is copied when no view has that shape."""
     _req(x.stride(-1) == 1, "inner dimension must be contiguous")
     if x.dim() == 2:
         return x, x.stride(0)
     x2 = x.reshape(-1, x.shape[-1])
+    return x2, x2.stride(0)
+
+
+def _out_rows2d(x):
+    """A tensor the kernel writes (out=, in-place operands) as a [rows, d] VIEW of its memory; returns (tensor2d, ld).
+    Raises ValueError when x's rows do not share one stride: the kernel would write a copy and x would never change."""
+    _req(x.stride(-1) == 1, "inner dimension must be contiguous")
+    if x.dim() == 2:
+        return x, x.stride(0)
+    try:
+        x2 = x.view(-1, x.shape[-1])
+    except RuntimeError:
+        raise ValueError(f"an output of shape {tuple(x.shape)} and strides {x.stride()} cannot be viewed as rows of one "
+                         "stride") from None
     return x2, x2.stride(0)
 
 
@@ -159,7 +173,7 @@ def gemm(a, w, bias=None, act=ACT_NONE, glu=GLU_NONE, residual=None, alpha=1.0, 
     else:
         _req(out.shape[-1] == n_out and out.stride(-1) == 1, "bad out shape")
         _req(out.dtype == (torch.float32 if out_fp32 else BF16), "bad out dtype")
-    out2, ldo = _rows2d(out)
+    out2, ldo = _out_rows2d(out)
     epi = Epilogue()
     epi.bias = _ptr(bias)
     epi.rowbias = _ptr(rowbias)
@@ -303,7 +317,7 @@ def rmsnorm(x, weight, eps, out=None):
     lib = _lib.load()
     x2, ldx = _rows2d(x)
     out = torch.empty_like(x) if out is None else out
-    o2, ldo = _rows2d(out)
+    o2, ldo = _out_rows2d(out)
     check(lib.vb200_rmsnorm(x2.data_ptr(), ldx, weight.data_ptr(), o2.data_ptr(), ldo, x2.shape[0], x2.shape[1],
                             float(eps), _stream()), "vb200_rmsnorm")
     _launches[0] += 1
@@ -315,7 +329,7 @@ def layernorm(x, weight, bias, eps, out=None):
     x2, ldx = _rows2d(x)
     if out is None:
         out = torch.empty(x.shape, dtype=BF16, device=x.device)
-    o2, ldo = _rows2d(out)
+    o2, ldo = _out_rows2d(out)
     check(lib.vb200_layernorm(x2.data_ptr(), ldx, weight.data_ptr(), _ptr(bias), o2.data_ptr(), ldo, x2.shape[0],
                               x2.shape[1], float(eps), _stream()), "vb200_layernorm")
     _launches[0] += 1
@@ -440,8 +454,9 @@ def add_rowgroup(x, table, group_rows, period, out=None):
     """x [rows, d] + table[(row // group_rows) % period]."""
     lib = _lib.load()
     x2, _ = _rows2d(x)
-    _req(x.is_contiguous() and table.is_contiguous(), "contiguous")
+    _req(x.is_contiguous() and table.is_contiguous() and x.dtype == BF16 and table.dtype == BF16, "contiguous bf16")
     out = torch.empty_like(x) if out is None else out
+    _req(out.shape == x.shape and out.dtype == BF16 and out.is_contiguous(), "out: contiguous bf16 of x's shape")
     check(lib.vb200_add_rowgroup(x2.data_ptr(), table.data_ptr(), out.data_ptr(), x2.shape[0], x2.shape[1],
                                  group_rows, period, _stream()), "vb200_add_rowgroup")
     _launches[0] += 1
@@ -451,7 +466,7 @@ def add_rowgroup(x, table, group_rows, period, out=None):
 def rope_kv_append(qkv, positions, n_heads, head_dim, theta, k_pages=None, v_pages=None, block_table=None,
                    batch_of_token=None, slot_of_token=None, page_size=0):
     lib = _lib.load()
-    q2, ld = _rows2d(qkv)
+    q2, ld = _out_rows2d(qkv)
     max_pages = block_table.shape[1] if block_table is not None else 0
     check(lib.vb200_rope_kv_append(q2.data_ptr(), ld, positions.data_ptr(), _ptr(batch_of_token),
                                    _ptr(slot_of_token), _ptr(k_pages), _ptr(v_pages), _ptr(block_table),
@@ -892,7 +907,7 @@ def layernorm_add(x, weight, bias, residual, eps, out=None):
     x2, ldx = _rows2d(x)
     if out is None:
         out = torch.empty(x.shape, dtype=BF16, device=x.device)
-    o2, ldo = _rows2d(out)
+    o2, ldo = _out_rows2d(out)
     r_ptr, ldr = 0, 0
     if residual is not None:
         r2, ldr = _rows2d(residual)
