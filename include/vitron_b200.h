@@ -95,10 +95,13 @@ int vb200_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void
  *   codes:  uint8 [N, ceil(K/128) * 64], 4-bit codes into bitsandbytes' nf4 table, in the kernel's byte order (nf4.py
  *           pack_codes); the row stride is implied by K;
  *   scales: fp16 [N, K / 64], one scale per (row, 64-column block): W_eff[n, k] = nf4[code] * float(scale[n, k / 64]).
- * vb200_gemm_nf4: out = epi(rowscale ⊙ (A · diag(kscale) · W_effᵀ)) with every vb_epilogue feature of vb200_gemm_bf16
- * (rms_eps computes the row scale from the raw A), for M <= 32 (else VB_ERR_UNSUPPORTED); kscale is an optional fp32
- * [K] column scale (16-byte aligned) applied to A in fp32 and rounded to bf16 before the products, which is how the
- * RMSNorm gain reaches a weight that was quantised unfolded. One launch, no workspace. lda multiple of 8.
+ * vb200_gemm_nf4: out = epi(rowscale ⊙ (Ã · W_tabᵀ)) with every vb_epilogue feature of vb200_gemm_bf16 (rms_eps
+ * computes the row scale from the raw A), for M <= 32 (else VB_ERR_UNSUPPORTED). W_tab[n, k] = bf16_rn(nf4[code]) *
+ * float(scale[n, k / 64]): the products use the NF4 values rounded to bf16 (up to 3.1e-3 relative from nf4[code], far
+ * below the quantisation error) and the scale multiplies each 64-block's fp32 sum, so the result is W_eff's only to
+ * that table rounding. kscale is an optional fp32 [K] column scale (16-byte aligned): Ã[m, k] = bf16_rn(A[m, k] *
+ * kscale[k]) in fp32, which is how the RMSNorm gain reaches a weight that was quantised unfolded (Ã = A without it).
+ * One launch, no workspace. lda multiple of 8, ldo >= N (N / 2 with a GLU).
  * vb200_nf4_dequant: out[N, K] bf16 (contiguous, 16-byte aligned) = bf16_rn((nf4[code] * scale) * kscale[k]), fp32
  * products in that order (kscale NULL = 1), bit-identical to nf4.py; larger M runs it into a workspace and then
  * vb200_gemm_bf16. Both follow the PDL rule of vb200_gemm_bf16's weight operand: codes, scales and kscale are

@@ -116,8 +116,13 @@ def test_argument_validation_without_device():
     assert lib.vb200_gemm_nf4(p, 96, p, p, None, p, 64, 1, 64, 96, C.byref(epi), None) == -1       # K % 64
     assert lib.vb200_gemm_nf4(p, 64, p, p, None, p, 64, 33, 64, 64, C.byref(epi), None) == -4      # M > 32
     assert lib.vb200_gemm_nf4(p, 64, p + 1, p, None, p, 64, 1, 64, 64, C.byref(epi), None) == -1   # misaligned codes
+    ks = C.cast(p + 4, C.POINTER(C.c_float))
+    assert lib.vb200_gemm_nf4(p, 64, p, p, ks, p, 64, 1, 64, 64, C.byref(epi), None) == -1         # misaligned kscale
+    assert lib.vb200_gemm_nf4(p, 68, p, p, None, p, 64, 1, 64, 64, C.byref(epi), None) == -1       # lda % 8 != 0
+    assert lib.vb200_gemm_nf4(p, 64, p, p, None, p, 63, 1, 64, 64, C.byref(epi), None) == -1       # ldo < N
     epi.glu = 1
     assert lib.vb200_gemm_nf4(p, 64, p, p, None, p, 64, 1, 48, 64, C.byref(epi), None) == -1      # GLU needs N % 32
+    assert lib.vb200_gemm_nf4(p, 64, p, p, None, p, 31, 1, 64, 64, C.byref(epi), None) == -1      # ldo < N / 2
     assert lib.vb200_nf4_dequant(None, p, None, p, 4, 64, None) == -1
     assert lib.vb200_nf4_dequant(p, p, None, p, 4, 100, None) == -1
     assert lib.vb200_nf4_dequant(p, p, None, p + 8, 4, 64, None) == -1

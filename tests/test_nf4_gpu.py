@@ -1,5 +1,7 @@
 """GPU: the NF4 kernels (csrc/gemv_nf4.cu) against the statement of vitron_b200/nf4.py, and an NF4 engine against a bf16
-engine that holds the same W_eff. Everything is compared with W_eff, never with the unquantised weights."""
+engine that holds the same W_eff. Everything is compared with W_eff, never with the unquantised weights. The kernels'
+float64 pins, with bounds derived from their arithmetic, every epilogue and the edge shapes, are in
+tests/test_nf4_kernels_gpu.py."""
 import pytest
 import torch
 

@@ -1,7 +1,14 @@
 // vitron_b200 — NF4 weight-streaming GEMM for M <= 32 tokens, and the NF4 -> bf16 dequantiser.
 //
-//   out[M, N'] = epilogue( rowscale ⊙ (X[M, K] · diag(kscale) · W_eff[N, K]^T) ),  M <= 32
-//   W_eff[n, k] = nf4[code(n, k)] * float(scale(n, k / 64))          (format: vitron_b200/nf4.py)
+//   out[M, N'] = epilogue( rowscale ⊙ (X~[M, K] · W_tab[N, K]^T) ),  M <= 32
+//   X~[m, k] = bf16_rn(float(X[m, k]) * kscale[k])   (X itself without kscale)
+//   W_tab[n, k] = bf16_rn(nf4[code(n, k)]) * float(scale(n, k / 64)), the scale applied in fp32 to each 64-block's sum
+//
+// W_tab is not the format's W_eff = nf4[code] * scale (vitron_b200/nf4.py): the table holds the NF4 values rounded to
+// bf16, which moves 13 of the 16 by up to 3.1e-3 relative (code 2), far below NF4's own quantisation error. Keeping the
+// fp32 values would cost the bf16x2 table lookup that feeds the mma directly. The dequantiser below rounds the other
+// product, bf16_rn(nf4[code] * scale * kscale[k]). tests/test_nf4_kernels_gpu.py pins the kernel against W_tab and bounds
+// its distance to W_eff.
 //
 // Decode is bound by weight bytes; 4-bit codes + one fp16 scale per (row, 64-block) stream 0.53 bytes per weight
 // instead of 2. The kernel follows gemv_bf16_kernel (gemv.cu): persistent, 2 CTAs per SM, each CTA owns 16 (32 for the

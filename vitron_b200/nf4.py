@@ -14,8 +14,10 @@ restates that quantisation with torch:
 Device format (`NF4Weight`): packed 4-bit codes and one fp16 scale per (row, 64-column block), the double-dequantised
 scale rounded to fp16. A per-row scale leaves the row order free, so q/k/v concatenation and the 16-row gate/up
 interleave of `ops.pack_glu_weight` apply to quantised rows as they do to bf16 ones. `dequantize` defines W_eff, the
-matrix every kernel result is compared with. Parity of this quantiser with bitsandbytes itself is not pinned (the
-library is not a dependency)."""
+matrix the format stands for. The dequantiser kernel rounds W_eff * kscale to bf16 bit for bit. The M <= 32
+weight-streaming kernel multiplies bf16_rn(NF4[code]) * scale instead, which is at most 3.1e-3 relative from W_eff;
+tests/test_nf4_kernels_gpu.py pins it against those operands and bounds its distance to W_eff. Parity of this quantiser
+with bitsandbytes itself is not pinned (the library is not a dependency)."""
 import torch
 
 NF4 = torch.tensor([-1.0, -0.6961928009986877, -0.5250730514526367, -0.39491748809814453, -0.28444138169288635,

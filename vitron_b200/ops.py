@@ -119,12 +119,12 @@ def _req(cond, msg):
 
 
 def _rows2d(x):
-    """An input x as [rows, d] with unit inner stride; returns (tensor2d, ld). x is copied when no view has that shape."""
+    """An input x as [rows, d] with unit inner stride; returns (tensor2d, ld). x is copied when no view has that shape.
+    A single row reports ld = d: torch gives a one-row tensor any row stride (a clone of a row of a padded buffer keeps
+    the buffer's), which the kernels' ld alignment checks would refuse although they never step to a second row."""
     _req(x.stride(-1) == 1, "inner dimension must be contiguous")
-    if x.dim() == 2:
-        return x, x.stride(0)
-    x2 = x.reshape(-1, x.shape[-1])
-    return x2, x2.stride(0)
+    x2 = x if x.dim() == 2 else x.reshape(-1, x.shape[-1])
+    return x2, (x2.stride(0) if x2.shape[0] > 1 else x2.shape[-1])
 
 
 def _out_rows2d(x):
@@ -154,9 +154,11 @@ def pack_glu_weight(w_a, w_b):
 
 def gemm(a, w, bias=None, act=ACT_NONE, glu=GLU_NONE, residual=None, alpha=1.0, rowbias=None,
          rowbias_rows=0, out=None, out_fp32=False, rowscale=None, rms_eps=0.0, kscale=None):
-    """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T) on wgmma tensor cores. w is bf16, or an NF4Weight (nf4.py): then
-    out = epilogue(a @ diag(kscale) @ W_eff^T) with the optional fp32 column scale kscale [K], on the NF4 weight-streaming
-    kernel for M <= 32 and as an NF4 -> bf16 dequantisation into a workspace followed by the bf16 GEMM above that."""
+    """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T) on wgmma tensor cores. w is bf16, or an NF4Weight (nf4.py) with the
+    optional fp32 column scale kscale [K]. For M <= 32 the NF4 weight-streaming kernel computes
+    epilogue(bf16_rn(a * kscale) @ W_tab^T), where W_tab = bf16_rn(NF4[code]) * scale differs from the format's W_eff by
+    the bf16 rounding of the 16 NF4 values (at most 3.1e-3 relative). Above that the weight is dequantised to
+    bf16_rn(W_eff * kscale) in a workspace and the bf16 GEMM multiplies a with it."""
     lib = _lib.load()
     a2, lda = _rows2d(a)
     q4 = isinstance(w, NF4Weight)
